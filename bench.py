@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — frames/s of the VToonify per-frame synthesis hot path on B200 (BASELINE.json metric).
+"""bench.py — frames/s of the VToonify per-frame synthesis hot path on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # this framework (N>1: launched by torchrun)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port) on the host cores
@@ -16,6 +16,8 @@ Default (configs[1]): a "step" is one ``VToonify.forward`` (+ clamp) over one ba
           inside the timed region, double-buffered (``ShardedFrameLoop``).  ``value``: the inputs start in rank 0's HBM and the
           frames end there; ``e2e``: they start and end in rank 0's pinned host memory.
 Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks.
+--dump-outputs DIR (single GPU): after the timed steps, the last timed step's output is written to DIR/<name>.npy (float32; a fixed,
+seeded sample of it when it is larger than the budget) so that two builds can be compared output for output on identical inputs.
 """
 import argparse
 import json
@@ -49,7 +51,7 @@ def load_peaks():
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet (dense, 700 W)"}
 
 
 class ClockSampler(threading.Thread):
@@ -200,13 +202,13 @@ def workload_config(cfg, args, world):
         return {"workload": f"StyleGAN2 Generator({cfg['size']}, 512, 8, 2) synthesis from W+ latents, fixed noise, batch {args.batch} per "
                             f"GPU per step ({cfg['name']})", "batch_per_gpu": args.batch, "units_per_step": world * args.batch,
                 "weights": "deterministic random-init (vtoonify_b200/weights.py)",
-                "l2": "every activation of the 256^2..1024^2 levels exceeds the 126 MB L2; no flush needed"}
+                "l2": "every activation of the 256^2..1024^2 levels exceeds the 50 MB L2; no flush needed"}
     H, W, B = args.height, args.width, args.batch
     return {"workload": f"VToonify-{'D' if cfg['backbone'] == 'dualstylegan' else 'T'} forward+clamp, "
                         f"{H}x{W} input frames -> {4 * H}x{4 * W}, batch {B} per GPU per step ({cfg['name']})",
             "backbone": cfg["backbone"], "batch_per_gpu": B, "frames_per_step": world * B,
             "weights": "deterministic random-init (vtoonify_b200/weights.py)",
-            "l2": f"inputs ({B * 22 * H * W * 4 / 1e6:.0f} MB) and every activation exceed the 126 MB L2; no flush needed"}
+            "l2": f"inputs ({B * 22 * H * W * 4 / 1e6:.0f} MB) and every activation exceed the 50 MB L2; no flush needed"}
 
 
 def run_reference(args, cfg, rank, world):
@@ -291,7 +293,7 @@ def run_cudnn(args, cfg, rank, world):
             "vs_baseline": None, "dtype": "tf32 (torch default: cudnn.allow_tf32=True)", "data": "synthetic",
             "config": workload_config(cfg, args, 1),
             "fp32": {"value": units / (res[False] * 1e-3), "ms_per_step": res[False], "note": "cudnn.allow_tf32=False"},
-            "custom_ops": ("the reference's own upfirdn2d / fused_bias_act CUDA kernels (oracle/_ref, compiled unmodified for sm_100a)"
+            "custom_ops": ("the reference's own upfirdn2d / fused_bias_act CUDA kernels (oracle/_ref, compiled unmodified for sm_90a)"
                            if ref_ops is not None else "pure-torch restatements of upfirdn2d / fused_bias_act (oracle/_ref not built)"),
             "note": f"oracle restatement of the reference graph on torch {torch.__version__} CUDA kernels (cuDNN {torch.backends.cudnn.version()}); "
                     "test infrastructure timed as a baseline, none of this repo's kernels on the path"}
@@ -312,13 +314,6 @@ def _roofline(prof, steps, ms, precision, peaks, cfg, units_per_rank_step, extra
     peak = peaks["bf16_tflops_sustained"]
     achieved = tc_flops / (tc_ms * 1e-3) / 1e12 if tc_ms > 0 else 0.0
     issued = tc_issued / (tc_ms * 1e-3) / 1e12 if tc_ms > 0 else 0.0
-    traffic = None
-    prof_json = os.path.join(ROOT, "profiles", "ncu_conv_tc_latest.json")
-    if os.path.exists(prof_json):
-        try:
-            traffic = json.load(open(prof_json)).get("dram_bytes_per_launch")
-        except Exception:
-            traffic = None
 
     def layer(k, v):
         t = v[0] * 1e-3
@@ -330,18 +325,18 @@ def _roofline(prof, steps, ms, precision, peaks, cfg, units_per_rank_step, extra
     top = [layer(k, v) for k, v in (ordered if extra_layers else ordered[:8])]
     products = {"bf16x3": 3, "tf32": 1, "fp32": 1}[precision]
     roof = {"bound": "tensor",
-            "kernel": ("conv_tc_kernel (tcgen05 kind::f16, fp32 operands split into bf16 hi+lo, 3 products, implicit-GEMM conv)"
-                       if precision == "bf16x3" else "conv_tc_kernel (tcgen05 kind::tf32 implicit-GEMM conv)"),
+            "kernel": ("conv_tc_kernel (wgmma bf16, fp32 operands split into bf16 hi+lo, 3 products, implicit-GEMM conv)"
+                       if precision == "bf16x3" else "conv_tc_kernel (wgmma tf32 implicit-GEMM conv)"),
             "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
             "frac_algorithmic": achieved / peak, "frac_issued": issued / peak,
-            "peak_note": f"{peaks['source']} dense bf16 cuBLAS throughput, sustained figure (the kernel is timed inside a long step); "
+            "peak_note": f"{peaks['source']} dense bf16 throughput; "
                          f"achieved counts ALGORITHMIC conv flops (2*MAC); frac_issued counts the bf16 MMA flops actually issued "
                          f"({products} products per algorithmic product, x4 for the folded up-convolutions)",
             "launches": len(prof), "kernel_ms_per_step": tc_ms / steps, "share_of_step": tc_ms / ms if ms > 0 else None,
             "hbm": {"algorithmic_gbs": tc_bytes / (tc_ms * 1e-3) / 1e9 if tc_ms > 0 else 0.0, "peak_gbs": peaks["hbm_gbs"],
                     "frac": tc_bytes / (tc_ms * 1e-3) / 1e9 / peaks["hbm_gbs"] if tc_ms > 0 else 0.0,
                     "note": "algorithmic bytes (inputs + outputs + weights of every conv launch, fp32) / conv kernel time; per layer in top_layers"},
-            "traffic": traffic, "top_layers": top}
+            "top_layers": top}
     if cfg["kind"] == "vtoonify":
         flop_unit = cfg["flop_per_px"] * cfg["H"] * cfg["W"]
         bytes_unit = cfg["bytes_per_px"] * cfg["H"] * cfg["W"]
@@ -419,11 +414,14 @@ def run_ours(args, cfg, rank, world, local_rank):
                 sampler.start()
             ops.set_tc_profile(prof)
             n0 = _lib.launch_count()
+            last = None
             e0.record()
             for _ in range(steps):
-                step()
+                last = step()
             e1.record()
             barrier()
+            if args.dump_outputs and rank == 0 and last is not None:
+                dump_outputs(args.dump_outputs, {"images" if is_gen else "frames": last})
         else:
             # ---- rank-0 clip: NCCL scatter -> forward -> NCCL gather of uint8 frames, inputs / results in rank 0's HBM
             dev_in = [h.to(dev) for h in hosts] if rank == 0 else None
@@ -518,10 +516,6 @@ def run_ours(args, cfg, rank, world, local_rank):
             for k, v in sorted(per.items(), key=lambda kv: -kv[1][0]):
                 f.write(f"{v[0] / steps:8.3f} ms  x{v[2] / steps:5.1f}  {v[1] / (v[0] * 1e-3) / 1e12:6.1f} TF/s alg  "
                         f"{v[4] / (v[0] * 1e-3) / 1e12:7.1f} TF/s issued  {v[3] / (v[0] * 1e-3) / 1e9:7.0f} GB/s alg  {k}\n")
-    if is_gen:
-        pj = os.path.join(ROOT, "profiles", "ncu_modconv_r02.json")
-        if os.path.exists(pj):
-            roofline["modconv_tensor_pipe_pct"] = json.load(open(pj))
     conf = workload_config(cfg, args, world)
     if world == 1 or is_gen:
         par = {"layout": f"{world} independent replica(s), no collective" if is_gen else "single GPU, inputs resident in HBM"}
@@ -654,6 +648,23 @@ def run_video(args, cfg, rank, world, local_rank):
     emit(json.dumps(line))
 
 
+DUMP_BUDGET_FLOATS = 8 << 20   # 32 MB of float32 per dumped array
+
+
+def dump_outputs(dirname, arrays):
+    """arrays: name -> tensor.  Written as float32 .npy; an array larger than the budget is replaced by a fixed sample of its
+    flattened elements (indices from a seeded generator, ascending), identical from run to run for the same shape."""
+    import numpy as np
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1).float()
+        if flat.numel() > DUMP_BUDGET_FLOATS:
+            idx = torch.randint(0, flat.numel(), (DUMP_BUDGET_FLOATS,), generator=torch.Generator().manual_seed(0)).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(dirname, name + ".npy"), flat.cpu().numpy().astype(np.float32))
+
+
 _REAL_STDOUT = None
 
 
@@ -688,6 +699,8 @@ def main():
     ap.add_argument("--ref-budget", type=float, default=660.0,
                     help="--impl reference: seconds the K timed CPU steps may take; full-size frames unless the host is too slow for that")
     ap.add_argument("--no-u8", action="store_true", help="skip the uint8-wire / on-device parsing end-to-end leg")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's output to DIR/<name>.npy (float32, seeded sample when large); single GPU")
     args = ap.parse_args()
     cfg = dict(CONFIGS[args.config])
     if args.backbone:
@@ -697,6 +710,8 @@ def main():
         cfg["W"] = args.width = args.width or cfg["W"]
     args.batch = args.batch or cfg["B"]
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
+    if args.dump_outputs and (args.impl != "ours" or args.config == "video" or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        ap.error("--dump-outputs needs the single-GPU timed path of this implementation (not --config video)")
 
     global _REAL_STDOUT
     sys.stdout.flush()

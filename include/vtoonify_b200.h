@@ -1,5 +1,5 @@
 /*
- * vtoonify_b200.h — C-ABI of libvtoonify_b200.so (hand-written sm_100a CUDA kernels).
+ * vtoonify_b200.h — C-ABI of libvtoonify_b200.so (hand-written sm_90a CUDA kernels).
  *
  * This is the drop-in boundary for the VToonify per-frame StyleGAN2 synthesis hot path.
  * Every entry point is `extern "C"`, takes plain device pointers + sizes + a CUDA stream
@@ -34,16 +34,18 @@
 extern "C" {
 #endif
 
-#define VT_ABI_VERSION 5   /* 2: vt_conv_desc gained weight_bf16x3 / bf16x3_nstack / src_scale, vt_smalln_desc src_mask / tsum, vt_split_weights_bf16x3
+#define VT_ABI_VERSION 6   /* 2: vt_conv_desc gained weight_bf16x3 / bf16x3_nstack / src_scale, vt_smalln_desc src_mask / tsum, vt_split_weights_bf16x3
                             * 3: face-parsing helpers (vt_frame_s2d_f32 .. vt_logits_readout_f32 with out_bstride), backward ops, frame pre-filter
                             * 4: row-strip kernels, vt_conv_desc gained split_fmt / acc_scale
                             * 5: vt_conv_desc gained stats_ws / stats_ws_floats (statistics of the conv output), vt_conv2d_tc_stats_chunks,
-                            *    vt_instnorm_finalize_f32 */
+                            *    vt_instnorm_finalize_f32
+                            * 6: sm_90a: vt_conv2d_rs takes the vt_conv2d_tc_tf32 weight split; the row-strip up-conv, vt_set_debug_buffer and
+                            *    vt_selftest_tc_gemm are gone */
 
 /* ---- library info / errors ------------------------------------------------------------- */
 int         vt_abi_version(void);
 const char* vt_last_error(void);          /* thread-local message of the last failing call   */
-const char* vt_build_info(void);          /* "sm_100a ... " build string                       */
+const char* vt_build_info(void);          /* "sm_90a ... " build string                        */
 /* number of kernel launches issued by this library since process start (all threads)        */
 int64_t     vt_launch_count(void);
 
@@ -107,7 +109,7 @@ int vt_fold_upconv_weights_f32(const float* w, const float* blur, float* out, in
  * becomes nstack_rows rows [hi|hi] followed by nstack_rows rows [lo|lo]. */
 int vt_split_weights_bf16x3(const float* w, void* out, int64_t rows, int C, int nstack_rows, void* stream);
 /* The same split with fp16 halves (11 + 11 mantissa bits): out = [half(w*scale) x 32 | half(w*scale - hi) x 32] per 32-channel chunk.
- * `scale` is a power of two that keeps the low halves out of fp16's subnormal range (undone by the consumer: vt_conv2d_rs acc_scale);
+ * `scale` is a power of two that keeps the low halves out of fp16's subnormal range (undone by the consumer: the descriptor's acc_scale);
  * |w * scale| must stay below 65504. */
 int vt_split_weights_f16x3(const float* w, void* out, int64_t rows, int C, float scale, void* stream);
 
@@ -189,42 +191,26 @@ typedef struct vt_conv_desc {
 
 /* fp32-exact CUDA-core implicit GEMM (FFMA). Any shape. */
 int vt_conv2d_direct_f32(const vt_conv_desc* d, void* stream);
-/* tcgen05 (TF32, fp32 accumulate in TMEM), TMA-staged tiles. Requires channel strides % 32 == 0,
- * Cout % 16 == 0, 16B-aligned views. */
+/* wgmma (TF32 or split 16-bit operands, fp32 accumulate in registers), TMA-staged tiles. Requires channel strides % 32 == 0,
+ * Cout % 32 == 0, 16B-aligned views. */
 int vt_conv2d_tc_tf32(const vt_conv_desc* d, void* stream);
 int vt_conv2d_tc_supported(const vt_conv_desc* d);   /* 1 if vt_conv2d_tc_tf32 accepts the descriptor */
 /* number of partial-sum chunks per (sample, channel) that vt_conv2d_tc_tf32 writes to desc->stats_ws for this descriptor under the current
  * options (-1 + vt_last_error() if the descriptor cannot produce statistics) */
 int vt_conv2d_tc_stats_chunks(const vt_conv_desc* d);
-/* Row-strip tensor-core kernel for the full-resolution 3x3 / stride 1 / padding 1 layers with Cin, Cout in {32, 64} (StyledConv conv2 of
- * the last generator levels, model/stylegan/model.py:298-304 + 364-392): the three vertical taps are stacked along the GEMM N dimension
- * and the partial sums of an output row are accumulated across input rows inside TMEM.  Same descriptor; `weight_bf16x3` must hold the
- * row-strip weight layout [wB][Cin/32][dx = -1,0,1][3*Cout rows: (dy = +1, 0, -1) x Cout][hi(32) | lo(32) 16-bit] and
- * `bf16x3_nstack` names the split format (2: bf16, 3: fp16).  Epilogue: v = acc * acc_scale + bias + noise_w * noise -> activation
- * (-> fused ToRGB tail).  Dense NHWC output only.  With the ToRGB tail present `out` may be NULL: only `rgb_out` is written (the
- * last StyledConv of the synthesis network: its activation has no reader, model/stylegan/model.py:549-556). */
+/* Row-strip layers: full-resolution 3x3 / stride 1 / padding 1 convolutions with Cin, Cout in {32, 64} (StyledConv conv2 of the last
+ * generator levels, model/stylegan/model.py:298-304 + 364-392).  Same descriptor and split weights as vt_conv2d_tc_tf32 (bf16x3 mode);
+ * acc_scale > 0 overrides desc->acc_scale.  With the fused ToRGB tail `out` may be NULL: only `rgb_out` is written (the last
+ * StyledConv of the synthesis network, whose activation has no reader: model/stylegan/model.py:549-556).  On sm_90a these layers run
+ * on the wgmma kernel. */
 int vt_conv2d_rs(const vt_conv_desc* d, float acc_scale, void* stream);
 int vt_conv2d_rs_supported(const vt_conv_desc* d);
-/* Row-strip UP-convolution (StyledConv up-layers, model/stylegan/model.py:273-286): out = Blur4x4(conv_transpose2d(in, w, stride 2)),
- * NHWC [B,H,W,Cin] -> [B,2H,2W,Cout], with only the horizontal half of the (separable) blur folded into the weights (2x the
- * algorithmic MACs instead of the 4x of vt_fold_upconv_weights_f32) and the vertical half applied to the TMEM accumulators.
- *   vt_fold_upconv_x_weights_f32: w9 [wB][9 = ky*3+kx][Cout][Cin] (modulated transposed-conv taps) + the FLIPPED 1-D blur taps
- *     g (4 HOST floats, K[m][n] = gk[m]*gk[n], g[m] = gk[3-m]) -> out [wB][Cout/32][Cin/32][3 (dx)][192 = (ky*2+px)*32+co][32]; split the
- *     result with vt_split_weights_bf16x3 / vt_split_weights_f16x3 (rows of 32 channels) and pass it as `w_split`.
- *   vt_conv_up2_rs: v = acc * acc_scale + bias + noise_w * noise[b, Y, X] -> activation; fmt 0 = bf16 split, 1 = fp16 split. */
-int vt_fold_upconv_x_weights_f32(const float* w9, const float* g_host4, float* out, int wB, int Cout, int Cin, void* stream);
-int vt_conv_up2_rs(const float* in, const void* w_split, float* out, int B, int H, int W, int Cin, int Cout, int wB,
-                   const float* g_host4, const float* bias, const float* noise, const float* noise_w, int act,
-                   float slope, float gain, int fmt, float acc_scale, void* stream);
-/* tuning knobs for experiments / tests: key in {"tc_mode","tc_mt","tc_tgroup","tc_cg2","tc_transpose","tc_pair_y","tc_direct_store","smalln_is","fir4","upfirdn_tiled","rs_cg","rs_rows","rs_strict","tc_strict","rsu_cg","rsu_rows",
+/* tuning knobs for experiments / tests: key in {"tc_mode","tc_mt","tc_tgroup","tc_transpose","smalln_is","fir4","upfirdn_tiled",
  * "tc_s2_halo","tc_stage_policy" (1: big halo boxes keep >= 5 weight stages), "tc_halo_pct" (halo staging threshold, % of the per-tap bytes),
- * "tc_warp_store" (1: per-warp output stores), "rsu_epi" (1: both output rows per epilogue pass), "rsu_bstages" (weight ring depth, 2..8),
- * "instnorm_chunks" (target chunks per sample on large maps, 0: small chunks)}; none of them changes results beyond fp32 rounding of the
- * instance-norm partial sums (tests/test_gpu_conv.py, tests/test_gpu_conv_rsu.py);
+ * "tc_m_major" (work-item order), "instnorm_chunks" (target chunks per sample on large maps, 0: small chunks)}; none of them changes results
+ * beyond fp32 rounding of the instance-norm partial sums (tests/test_gpu_conv.py);
  * returns the previous value (-1 for an unknown key) */
 int vt_set_option(const char* key, int value);
-/* tuning only: device buffer of 148*16 uint64 that conv_tc fills with per-role wait-cycle counters (NULL disables) */
-int vt_set_debug_buffer(void* dev_ptr);
 
 /* ---- small-N conv (Cout <= 4): planar output, optional planar extra source + skip upsample */
 typedef struct vt_smalln_desc {
@@ -327,11 +313,6 @@ int vt_frame_resize_crop_u8(const uint8_t* in, uint8_t* out, int B, int Hs, int 
 int vt_frame_u8_to_f32(const uint8_t* in, float* out, int B, int H, int W, int swap_rb, int64_t out_batch_stride, void* stream);
 /* fp32 NCHW (3ch) -> clamp(-1,1) -> ((v+1)*127.5) truncated to u8, HWC, optional RGB->BGR ; util.py:190-192 */
 int vt_f32_to_frame_u8(const float* in, uint8_t* out, int B, int H, int W, int swap_rb, void* stream);
-
-/* ---- tcgen05 issue-rate microbenchmark (tools/ only): D[0] = average SM cycles per tcgen05.mma (M=128, N, K=8 tf32)
- * over K*4 MMAs on resident smem operands. variant bit0: alternate 2 accumulators, bit1: converged-warp issue,
- * bit2: commit+wait per 4 MMAs. A, B, M unused. */
-int vt_selftest_tc_gemm(const float* A, const float* Bm, float* D, int M, int N, int K, int variant, void* stream);
 
 #ifdef __cplusplus
 }

@@ -162,6 +162,8 @@ def golden_vtoonify():
         # zplus2wplus
         z = torch.randn((1, 18, 512), generator=gen(9))
         out["zplus"], out["wplus"] = z, m.zplus2wplus(z)
+        # the input frames go to a file of their own: together with the outputs they exceed 1 MB
+        save(f"vtoonify_{tag}_x", **{k: out.pop(k) for k in ("a_x", "b_x")})
         save(f"vtoonify_{tag}", **out)
 
 

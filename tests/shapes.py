@@ -75,3 +75,12 @@ def layer_template(kind, name):
 def layer_state_dict(kind, name):
     seed = 3 if kind == "Generator32" else 7
     return det_state_dict(layer_template(kind, name), seed=seed)
+
+
+def vtoonify_golden(golden, tag):
+    """the VToonify-{tag} goldens: outputs / styles and, stored apart, the input frames (a_x, b_x)"""
+    g = golden(f"vtoonify_{tag}")
+    out = {k: g[k] for k in g.files}
+    gx = golden(f"vtoonify_{tag}_x")
+    out.update({k: gx[k] for k in gx.files})
+    return out

@@ -36,9 +36,9 @@ def test_library_exports_every_declared_symbol():
 def test_load_binds_and_reports_version():
     from vtoonify_b200 import _lib
     lib = _lib.load()
-    assert lib.vt_abi_version() == _lib.ABI_VERSION == 5
-    assert b"abi=5" in lib.vt_build_info()
-    assert b"sm_100a" in lib.vt_build_info()
+    assert lib.vt_abi_version() == _lib.ABI_VERSION == 6
+    assert b"abi=6" in lib.vt_build_info()
+    assert b"sm_90a" in lib.vt_build_info()
     assert ctypes.sizeof(_lib.ConvDesc) % 8 == 0
 
 
@@ -111,12 +111,12 @@ def _plan_desc(B, Cin, Cout, H, W, k=3, dil=1):
 
 
 def test_output_statistics_plan_is_host_only_and_batch_independent():
-    """vt_conv2d_tc_stats_chunks plans without touching the GPU: one chunk per (pixel tile of an image, CTA of a pair, M tile of
-    the work item, epilogue warp); the plan must not depend on the batch size (a frame's statistics may not depend on its batch)."""
+    """vt_conv2d_tc_stats_chunks plans without touching the GPU: one chunk per (pixel tile of an image, M tile of the work item,
+    consumer warp); the plan must not depend on the batch size (a frame's statistics may not depend on its batch)."""
     from vtoonify_b200 import _lib
     lib = _lib.load()
-    # 72 x 128 maps are handed over transposed: 9 x 8 tiles of 8 x 16 pixels = 36 pair items x 2 CTAs x 4 warps
-    assert lib.vt_conv2d_tc_stats_chunks(ctypes.byref(_plan_desc(4, 512, 512, 72, 128))) == 288
+    # 72 x 128 maps are handed over transposed: 9 x 8 tiles of 8 x 16 pixels x 8 consumer warps of 16 pixels
+    assert lib.vt_conv2d_tc_stats_chunks(ctypes.byref(_plan_desc(4, 512, 512, 72, 128))) == 576
     for shape in [(512, 512, 72, 128, 3, 1), (512, 512, 72, 128, 3, 4), (64, 128, 19, 45, 3, 1), (128, 32, 16, 24, 1, 1), (32, 64, 9, 7, 3, 1)]:
         n = [lib.vt_conv2d_tc_stats_chunks(ctypes.byref(_plan_desc(B, *shape))) for B in (1, 2, 4, 7)]
         assert n[0] > 0 and len(set(n)) == 1, (shape, n)

@@ -1,4 +1,4 @@
-"""GPU parity of the convolution kernels: fp32 FFMA kernel vs the oracle's F.conv2d; tcgen05 kernel vs the FFMA kernel
+"""GPU parity of the convolution kernels: fp32 FFMA kernel vs the oracle's F.conv2d; wgmma kernel vs the FFMA kernel
 on TF32-representable data (where both must agree to fp32 accumulation-order noise), for every staging mode."""
 import numpy as np
 import pytest
@@ -231,7 +231,8 @@ def test_folded_upconv(shape):
 @pytest.mark.parametrize("case", [CASES[1], CASES[2], CASES[3], CASES[4], CASES[5], (2, 256, 256, 40, 24, 3, 1, 1, 1), (1, 512, 512, 16, 16, 3, 1, 4, 4),
                                   (2, 64, 256, 17, 9, 3, 1, 1, 1), (2, 32, 32, 33, 70, 3, 1, 1, 1)])
 def test_tc_cta_pairs(case, cg2):
-    """cta_group::2 (CTA pair, M = 256) vs single-CTA tcgen05 vs the FFMA kernel on N-tile-256 layers."""
+    """The tensor-core kernel vs the FFMA kernel on Cout-256 layers (the "tc_cg2" key of the Blackwell CTA-pair build is unknown
+    to the Hopper library: every parameter set runs the single-CTA kernel)."""
     from vtoonify_b200 import _lib, ops
     B, Cin, Cout, H, W, k, stride, pad, dil = case
     g = torch.Generator().manual_seed(hash(case) % 10007)
@@ -335,8 +336,8 @@ def test_bf16x3_folded_upconv_and_concat(shape):
 @pytest.mark.parametrize("case", [CASES[2], CASES[3], CASES[4], CASES[5], (2, 32, 32, 33, 20, 3, 1, 1, 1), (1, 64, 64, 9, 40, 1, 1, 0, 1),
                                   (1, 512, 512, 24, 16, 3, 1, 1, 1)])
 def test_tc_transposed_view_and_pair_orientation(case, transpose, pair_y):
-    """The planner may hand the problem to the kernel transposed (x <-> y) and stack CTA pairs along y; both are pure
-    re-indexings and must not change results (noise, residual and bias exercise every strided epilogue read)."""
+    """The planner may hand the problem to the kernel transposed (x <-> y), a pure re-indexing that must not change results (noise,
+    residual and bias exercise every strided epilogue read); "tc_pair_y" is a key of the Blackwell CTA-pair build, ignored here."""
     from vtoonify_b200 import _lib, ops
     B, Cin, Cout, H, W, k, stride, pad, dil = case
     g = torch.Generator().manual_seed(hash(case) % 10007 + 5)
@@ -672,7 +673,7 @@ def test_instnorm_chunk_plans_agree(shape):
         assert (s1 - res[0][1]).abs().max().item() <= 2e-6 * max(1.0, res[0][1].abs().max().item()), plan
 
 
-@pytest.mark.parametrize("case", [(4, 512, 512, 72, 128, 3, 1, 1, 1),    # the res-block layer (transposed view, CTA pairs, 2 N tiles)
+@pytest.mark.parametrize("case", [(4, 512, 512, 72, 128, 3, 1, 1, 1),    # the res-block layer (transposed view, 2 N tiles)
                                   (2, 512, 512, 24, 40, 3, 1, 4, 4),     # dilation 4
                                   (2, 64, 128, 19, 45, 3, 1, 1, 1),      # 2 M tiles per work item, partial tiles
                                   (1, 128, 32, 16, 24, 1, 1, 0, 1),      # 1x1, N = 32 (4 M tiles per work item)

@@ -1,5 +1,6 @@
-"""Row-strip tensor-core kernel (csrc/conv_rs.cu: vertical taps stacked along N, cross-row accumulation in a TMEM slot ring)
-against the fp32 FFMA kernel and against the tap-by-tap tensor-core kernel on the same descriptors."""
+"""Row-strip entry point (vt_conv2d_rs: the full-resolution 3x3 layers with Cin, Cout in {32, 64}, including the image-only ToRGB
+launch) against the fp32 FFMA kernel and against the tap-by-tap tensor-core route on the same descriptors.  The "rs_cg" / "rs_rows"
+keys belong to the Blackwell row-strip kernel and are unknown to the sm_90a library."""
 import pytest
 import torch
 

@@ -1,5 +1,6 @@
-"""Row-strip up-convolution kernel (csrc/conv_rsu.cu: Blur o conv_transpose2d with the horizontal blur folded into the weights and
-the vertical blur applied to the TMEM accumulators) against the fp32 polyphase transposed conv + FIR pass and the folded kernel."""
+"""Row-strip up-convolution entry point (ops.conv_up2_rs_nhwc: Blur o conv_transpose2d as one convolution over the 4 output
+phases) against the fp32 polyphase transposed conv + FIR pass and the folded route.  The "rsu_*" keys belong to the Blackwell
+row-strip kernel and are unknown to the sm_90a library."""
 import pytest
 import torch
 

@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 import torch
 
+from tests.shapes import vtoonify_golden
+
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 
@@ -34,7 +36,7 @@ def model(request):
 def test_forward_golden(golden, model, prec):
     from vtoonify_b200 import ops
     tag, m = model
-    g = golden(f"vtoonify_{tag}")
+    g = vtoonify_golden(golden, tag)
     ops.set_precision(prec)
     try:
         for case in ("a", "b"):
@@ -58,7 +60,7 @@ def test_forward_golden(golden, model, prec):
 
 def test_aux_paths(golden, model):
     tag, m = model
-    g = golden(f"vtoonify_{tag}")
+    g = vtoonify_golden(golden, tag)
     w = m.zplus2wplus(T(g["zplus"]).cuda())
     assert (w.cpu() - T(g["wplus"])).abs().max().item() <= 5e-5
     x, style = T(g["b_x"]).cuda(), T(g["b_style"]).cuda()
@@ -80,7 +82,7 @@ def test_style_cache(golden, model):
     from vtoonify_b200 import _lib
     from vtoonify_b200.weights import det_state_dict
     tag, m = model
-    g = golden(f"vtoonify_{tag}")
+    g = vtoonify_golden(golden, tag)
     x = T(g["a_x"]).cuda()                                           # B = 2
     style = T(g["a_style"])[:1].repeat(2, 1, 1).cuda()              # one video, one style: both rows carry the same code
     y_first = m(x, style, d_s=0.5)

@@ -8,7 +8,7 @@ import torch
 
 from oracle import vt_oracle as O
 from vtoonify_b200.weights import det_state_dict
-from tests.shapes import layer_state_dict
+from tests.shapes import layer_state_dict, vtoonify_golden
 
 torch.set_grad_enabled(False)
 
@@ -90,7 +90,7 @@ def test_generator_golden(golden):
 
 @pytest.mark.parametrize("tag,backbone", [("d", "dualstylegan"), ("t", "toonify")])
 def test_vtoonify_golden(golden, tag, backbone):
-    g = golden(f"vtoonify_{tag}")
+    g = vtoonify_golden(golden, tag)
     keys = json.load(open(f"tests/golden/state_dict_keys_{tag}.json"))
     sd = det_state_dict({k: torch.empty(v) for k, v in keys.items()}, seed=0)
     # FIR buffers are architecture constants, not random (weights.py keeps the template value)

@@ -1,4 +1,4 @@
-"""vtoonify_b200 — B200-native (sm_100a) implementation of VToonify's per-frame StyleGAN2 synthesis hot path.
+"""vtoonify_b200 — H100-native (sm_90a) implementation of VToonify's per-frame StyleGAN2 synthesis hot path.
 
 Drop-in surface (same names / signatures / state_dict keys as the reference):
   vtoonify_b200.op            <-> model/stylegan/op   (upfirdn2d, fused_leaky_relu, FusedLeakyReLU, conv2d_gradfix)

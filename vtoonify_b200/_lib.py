@@ -10,7 +10,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvtoonify_b200.so")
-ABI_VERSION = 5
+ABI_VERSION = 6
 VT_MAX_TAPS = 36
 ACT_NONE, ACT_LRELU, ACT_RELU_TANH = 0, 1, 2
 
@@ -84,11 +84,7 @@ SYMBOLS = {
     "vt_conv2d_tc_supported": (c_int, [POINTER(ConvDesc)]),
     "vt_conv2d_rs": (c_int, [POINTER(ConvDesc), c_float, _P]),
     "vt_conv2d_rs_supported": (c_int, [POINTER(ConvDesc)]),
-    "vt_fold_upconv_x_weights_f32": (c_int, [_P, POINTER(c_float), _P, c_int, c_int, c_int, _P]),
-    "vt_conv_up2_rs": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_float), _P, _P, _P, c_int, c_float, c_float,
-                               c_int, c_float, _P]),
     "vt_set_option": (c_int, [c_char_p, c_int]),
-    "vt_set_debug_buffer": (c_int, [_P]),
     "vt_smalln_conv_f32": (c_int, [POINTER(SmallNDesc), _P]),
     "vt_affine_fold_weights_f32": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),
     "vt_fir_nhwc_f32": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, c_int,
@@ -110,7 +106,6 @@ SYMBOLS = {
     "vt_frame_resize_crop_u8": (c_int, [_P, _P] + [c_int] * 9 + [_P, _P, _P]),
     "vt_frame_u8_to_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int64, _P]),
     "vt_f32_to_frame_u8": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
-    "vt_selftest_tc_gemm": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
 }
 
 _lib = None
@@ -132,8 +127,8 @@ def load():
         fn.argtypes = args
     if lib.vt_abi_version() != ABI_VERSION:
         raise VtError(f"ABI mismatch: library reports {lib.vt_abi_version()}, binding expects {ABI_VERSION}")
-    for env, key in (("VT_TC_MODE", b"tc_mode"), ("VT_TC_MT", b"tc_mt"), ("VT_TC_TGROUP", b"tc_tgroup"), ("VT_TC_CG2", b"tc_cg2"),
-                     ("VT_TC_DIRECT_STORE", b"tc_direct_store"), ("VT_TC_STRICT", b"tc_strict"), ("VT_TC_STAGE_POLICY", b"tc_stage_policy"), ("VT_TC_HALO_PCT", b"tc_halo_pct"), ("VT_RS_STRICT", b"rs_strict"), ("VT_RSU_EPI", b"rsu_epi"), ("VT_TC_WARP_STORE", b"tc_warp_store"), ("VT_TC_M_MAJOR", b"tc_m_major"),
+    for env, key in (("VT_TC_MODE", b"tc_mode"), ("VT_TC_MT", b"tc_mt"), ("VT_TC_TGROUP", b"tc_tgroup"),
+                     ("VT_TC_STAGE_POLICY", b"tc_stage_policy"), ("VT_TC_HALO_PCT", b"tc_halo_pct"), ("VT_TC_M_MAJOR", b"tc_m_major"),
                      ("VT_INSTNORM_CHUNKS", b"instnorm_chunks")):
         if os.environ.get(env) is not None and os.environ.get(env) != "":
             lib.vt_set_option(key, int(os.environ[env]))      # tuning experiments only

@@ -19,8 +19,8 @@ int vt_num_sms() {
   static int sms = 0;
   if (sms == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -31,7 +31,7 @@ const char* vt_last_error(void) { return g_err; }
 const char* vt_build_info(void) {
 #define VT_STR2(x) #x
 #define VT_STR(x) VT_STR2(x)
-  return "libvtoonify_b200 abi=" VT_STR(VT_ABI_VERSION) " arch=sm_100a cuda="
+  return "libvtoonify_b200 abi=" VT_STR(VT_ABI_VERSION) " arch=sm_90a cuda="
       VT_STR(__CUDACC_VER_MAJOR__) "." VT_STR(__CUDACC_VER_MINOR__) " built " __DATE__;
 }
 int64_t vt_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }

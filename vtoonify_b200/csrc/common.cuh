@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for libvtoonify_b200 (sm_100a only).
+// common.cuh — shared helpers for libvtoonify_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,8 +6,8 @@
 #include <stdarg.h>
 #include "../../include/vtoonify_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libvtoonify_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libvtoonify_b200 is written for sm_90a (H100) only"
 #endif
 
 int vt_set_error(const char* fmt, ...);

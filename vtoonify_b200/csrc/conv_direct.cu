@@ -1,7 +1,7 @@
 // conv_direct.cu — fp32-exact CUDA-core convolutions on NHWC activations.
 //
 //   vt_conv2d_direct_f32 : implicit-GEMM FFMA kernel (64 pixels x 64 couts x 16 k per CTA, 4x4 register tile).
-//                          It is the fp32 reference-grade path ("precision=fp32") used to cross-check the tcgen05
+//                          It is the fp32 reference-grade path ("precision=fp32") used to cross-check the wgmma
 //                          kernel on the GPU and to run shapes the tensor-core kernel does not take.
 //   vt_smalln_conv_f32   : Cout <= 4 convolutions (ToRGB 1x1, fusion_skip 3x3, Fusion mask 3x3, encoder[-1] 1x1).
 //                          These are < 0.4 % of the FLOPs but read the largest tensors (SURVEY.md App. B), so they
@@ -15,7 +15,7 @@
 // a transposed stride-2 conv is issued as 4 polyphase calls (tap lists with dy,dx in {0,-1}) into a strided view.
 #include "common.cuh"
 
-int g_smalln_is = 1;   // input-stationary kernel for 3x3 small-N convolutions: 1 = where measured faster, 2 = always, 0 = never
+int g_smalln_is = 1;   // input-stationary kernel for 3x3 small-N convolutions: 1 = automatic (Cout == 1 on large maps), 2 = always, 0 = never
 
 namespace {
 
@@ -660,7 +660,7 @@ extern "C" int vt_smalln_conv_f32(const vt_smalln_desc* d, void* stream) {
   VT_CHECK(d->src_c == 0 || d->w_cstride >= cw, "smalln_conv: weight row shorter than the (virtual-concat) channel count");
   cudaStream_t st = (cudaStream_t)stream;
   // input-stationary kernel for 9-tap convolutions whose taps stay within +-2 pixels
-  // (measured on B200: faster than the gather kernel for Cout == 1 on maps of >= 64 patches, slower for Cout >= 2)
+  // (chosen automatically for Cout == 1 on maps of >= 64 patches only)
   const bool is_auto = d->Cout == 1 && vt_cdiv(d->W, IS_PW) * vt_cdiv(d->H, IS_PH) >= 64;   // per image: the choice must not depend on the batch size (frames are independent units)
   if ((g_smalln_is == 2 || (g_smalln_is == 1 && is_auto)) && d->taps == IS_TAPS && d->src_c >= 32) {
     int dy0 = 0, dy1 = 0, dx0 = 0, dx1 = 0;

@@ -1,17 +1,18 @@
-// conv_tc.cu — the hot kernel: NHWC convolution as an implicit GEMM on the 5th-gen tensor cores.
+// conv_tc.cu — the hot kernel: NHWC convolution as an implicit GEMM on the Hopper tensor cores (wgmma).
 //
-//   D[128 pixels, N couts] (TMEM, fp32) += A[128 pixels, 32 ch] (smem, TF32) * W[N couts, 32 ch]^T (smem, TF32)
+//   D[128 pixels, N couts] (registers, fp32) += A[128 pixels, 32 ch] (smem, TF32) * W[N couts, 32 ch]^T (smem, TF32)
 //
-// One persistent CTA per SM, warp-specialised:
+// One persistent CTA per SM, three warpgroups:
 //   warp 0 (1 lane)  TMA producer : activation tiles are 4-D boxes (32 ch, 8 x, 16 y, 1 b) of the NHWC tensor, shifted by
 //                                   the filter tap; out-of-image pixels are zero-filled by TMA == the conv's zero padding,
 //                                   so there is no im2col buffer and no bounds code.  Weight tiles are (32 ch, N, 1 tap, 1 b)
 //                                   boxes of the per-sample modulated/demodulated weights [b][tap][cout][cin].
-//   warp 1 (1 lane)  MMA issuer   : tcgen05.mma.cta_group::1.kind::tf32, M=128, N<=256, K=8 x4 per 128-byte swizzle row,
-//                                   accumulators double-buffered in TMEM so the epilogue of tile i overlaps the mainloop of i+1.
-//   warp 2           TMEM alloc / dealloc
-//   warps 4-7        epilogue     : tcgen05.ld 32 columns at a time -> (+noise, +bias, leaky-relu*gain, residual, TF32 rna) ->
-//                                   128B-swizzled smem staging -> TMA store (clips partial tiles).
+//   warps 1-3        operand transform (bf16x3 only): fp32 rows -> [hi | lo] 16-bit rows, in place.
+//   warpgroups 1, 2  consumers    : each owns 64 of the 128 pixels (8 rows of the 8 x 16 tile): wgmma m64nNk8 (tf32) or
+//                                   m64nNk16 (bf16 / fp16 split operands, N <= 128), fp32 accumulators in registers, one wgmma group
+//                                   kept in flight while the next stage is awaited; then the epilogue straight from the
+//                                   accumulator registers (+noise, +bias, leaky-relu*gain, residual, TF32 rna, fused ToRGB,
+//                                   instance-norm partial sums) with direct global stores.
 //
 // A-operand reuse ("halo" mode, stride-1 convs): one TMA box of (8+2d) x (16+2d) pixels per 32-channel chunk serves all
 // 9 taps; each tap's MMA reads it through a descriptor whose start address is shifted by whole 128-byte rows and whose
@@ -36,40 +37,39 @@ namespace {
 
 constexpr int TILE_W = 8, TILE_H = 16, TILE_M = 128;
 constexpr int KCH = 32;                       // fp32 channels per K chunk = one 128-byte swizzle row
-constexpr int STAGING_BYTES = TILE_M * 128;   // one 32-column output chunk
 constexpr int MAX_SMEM = 227 * 1024;
+constexpr int MAX_BLOCK_N = 128;              // largest N tile (wgmma N) of one work item
+constexpr int MAX_ACC_COLS = 128;             // accumulator columns per consumer thread group: mt * mma_n (64 registers; 128 spill)
+constexpr int STATS_WARPS = 8;                // instance-norm chunks per 128-pixel tile: one per consumer warp (16 pixels)
 
 struct TcArgs {
   CUtensorMap in_map[2][4];
   CUtensorMap w_map;
-  CUtensorMap out_map[4];                      // one strided output view per phase
   int n_src, kchunks[2], coff[2];
   // "B steps": one weight tile (tap of one phase) each; every step feeds `mt` accumulators (the M tiles of the work item)
   int n_steps;
   int8_t step_view[VT_MAX_TAPS], step_vx[VT_MAX_TAPS], step_vy[VT_MAX_TAPS];
   int16_t step_w[VT_MAX_TAPS];
   int step_aoff[VT_MAX_TAPS];                  // halo mode: byte offset of the tap's first row inside the halo box
-  int mt, n_phase, acc_stages;                 // mt accumulators (M tiles) of block_n columns per work item; n_phase: the N
+  int mt, n_phase;                             // mt accumulators (M tiles) of block_n columns per work item; n_phase: the N
                                                // dimension is phase-major [n_phase][Cout] (folded up-conv), else 1
   int tgroup;                                  // taps per weight TMA box / pipeline step (consecutive slabs)
-  int grp_first_mask, grp_last_mask;           // bit t: tap t is the first / last of its weight box (n_steps <= 32)
   int halo, halo_x0, halo_y0, halo_w;   // halo staging; x0/y0/w describe view 0's box (stride 1: the only one)
   // halo boxes of one K chunk: stride 1 has one, stride 2 one per parity view in use (each with its own extent and pitch)
   int n_hv, hv_view[4], hv_x0[4], hv_y0[4], hv_off[4], hv_bytes[4], a_rows;
   uint16_t step_sbo[VT_MAX_TAPS];   // halo mode: stride (bytes) between 8-pixel row groups of the tap's box
   int a_stages, b_stages, a_stage_bytes, b_stage_bytes, a_tx_bytes, b_tx_bytes;
-  int block_n, n_tiles, tiles_x, tiles_y, B, total_tiles, tmem_cols;
+  int block_n, n_tiles, tiles_x, tiles_y, B, total_tiles;
   int Ho, Wo, Cout, wB, out_cpitch;
   const float* bias;
   const float* noise;
   const float* noise_w;
   const float* res;
-  float* out;                // output base (direct-store epilogue; the TMA path goes through out_map)
+  float* out;
   int64_t out_sb, out_sy, out_sx, phase_off[4];
   int64_t pix_sb, pix_sy, pix_sx, phase_pix[4];   // the same view in dense-pixel units (noise index), = offsets / out_cpitch
   int act, round_tf32;
   float slope, gain, alpha, beta;
-  unsigned long long* dbg;   // optional [grid][16] cycle counters (tuning only)
   // fused ToRGB tail
   const float* rgb_w; const float* rgb_bias; const float* rgb_skip; const float* rgb_skip_kernel; float* rgb_out;
   const float* slope_vec;
@@ -78,596 +78,451 @@ struct TcArgs {
   int src_cn[2];             // channels of source s (row length of src_affine)
   int64_t sc_sb, sc_sy, sc_sx;
   int in_w, in_h;            // kernel-space input extents
-  int mma_n;                 // N of one MMA / TMEM columns per accumulator: block_n, or 2*block_n in the N-stacked bf16x3 form
+  int mma_n;                 // N of one MMA: block_n, or 2*block_n in the N-stacked bf16x3 form
   int nstack;                // bf16x3, Cout == 32: weight rows [w_hi|w_hi] x32 then [w_lo|w_lo] x32 -> 4 MMAs per tap, halves summed in the epilogue
-  int m_major;               // work-item order: the N tiles of one pixel tile are neighbours (run on neighbouring CTA pairs at the
-                             // same time, so the second read of the activations hits L2) instead of N-tile-major
+  int m_major;               // work-item order: the N tiles of one pixel tile are neighbours (run on neighbouring SMs at the same
+                             // time, so the second read of the activations hits L2) instead of N-tile-major
   float* stats_ws;           // optional instance-norm partial sums of the OUTPUT: [chunk][B][Cout][2] (sum, sum of squares), one chunk per
-                             // (pixel tile, epilogue warp); finalised by vt_instnorm_finalize_f32
-  int warp_store;            // epilogue: every warp stages and TMA-stores its own 32 pixels (8 x 4 box), no CTA-wide barrier
-  int direct_store;          // epilogue writes its 128-byte pixel rows straight to global memory instead of smem staging + TMA store
-  int pair_y;                // CG == 2: the CTA pair is stacked along y (rows) instead of x
+                             // (pixel tile, consumer warp); finalised by vt_instnorm_finalize_f32
   int bf16x3;                // operands split into bf16 hi/lo in shared memory, 3 MMA products (fp32-class accuracy)
-  int strict_release;        // 1: cluster-scope release on the transform warps' remote arrive (A/B switch)
   int fmt;                   // split-operand format: 0 = bf16 hi/lo, 1 = fp16 hi/lo
   float acc_scale;           // accumulators are multiplied by this first (undoes the power-of-two weight scale of the fp16 split)
 };
 
-#define VT_TWAIT(slot, stmt) do { if (p.dbg) { const long long t__ = clock64(); stmt; tw[slot] += clock64() - t__; } else { stmt; } } while (0)
+constexpr int TC_THREADS = 384;
+constexpr int XFORM_WARPS = 3;
+constexpr int CONSUMERS = 2;
+// wgmma.wait_group covers the executing warp's share of a warpgroup MMA only: every consumer warp releases a stage it has read
+constexpr int RELEASE_ARRIVALS = CONSUMERS * 4;
 
-// CG = 1: one CTA per work item (M = 128).  CG = 2: a CTA pair (cluster of 2) shares one tcgen05.mma.cta_group::2 with
-// M = 256: each CTA stages the activations of its own 128 pixels and HALF of every weight tile, so per-SM shared-memory
-// traffic (TMA writes + tensor-core operand reads) drops from ~160 to ~100 B/clk; rank 0 issues the MMAs for both.
-// warps: 0 TMA producer, 1 MMA issuer, 2-3 and 8-9 operand transform (bf16x3), 2 also TMEM alloc, 4-7 epilogue
-constexpr int TC_THREADS = 320;
-constexpr int XFORM_WARPS = 4;
+// one K step of one accumulator: the products of a 32-channel chunk (4 tf32 MMAs, or the split-operand MMAs)
+template <int NW>
+__device__ __forceinline__ void mma_step(float* acc, uint64_t adesc, uint64_t bdesc, uint32_t first, int bf16x3, int fmt, int nstack) {
+  if (!bf16x3) {
+    if constexpr (NW == 32) {
+      wgmma_tf32_n32(acc, adesc, bdesc, first ^ 1u); wgmma_tf32_n32(acc, adesc + 2, bdesc + 2, 1);
+      wgmma_tf32_n32(acc, adesc + 4, bdesc + 4, 1); wgmma_tf32_n32(acc, adesc + 6, bdesc + 6, 1);
+    } else if constexpr (NW == 64) {
+      wgmma_tf32_n64(acc, adesc, bdesc, first ^ 1u); wgmma_tf32_n64(acc, adesc + 2, bdesc + 2, 1);
+      wgmma_tf32_n64(acc, adesc + 4, bdesc + 4, 1); wgmma_tf32_n64(acc, adesc + 6, bdesc + 6, 1);
+    } else {
+      wgmma_tf32_n128(acc, adesc, bdesc, first ^ 1u); wgmma_tf32_n128(acc, adesc + 2, bdesc + 2, 1);
+      wgmma_tf32_n128(acc, adesc + 4, bdesc + 4, 1); wgmma_tf32_n128(acc, adesc + 6, bdesc + 6, 1);
+    }
+    return;
+  }
+  // The A row is [a_hi(32)|a_lo(32)] and the B row [w_hi(32)|w_lo(32)] 16-bit; +2 on a descriptor = +32 B = 16 elements of K.
+  //   nstack:  [a_hi|a_lo] (K = 64) x rows [w_hi|w_hi] (columns 0..31) and [w_lo|w_lo] (columns 32..63): all four products
+  //   else:    a*w ~= a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the dropped a_lo*w_lo term is ~2^-18 relative)
+  const int ao[6] = {0, 2, 4, 6, 0, 2};
+  const int bo[6] = {0, 2, 0, 2, 4, 6};
+  const int n = nstack ? 4 : 6;
+#define VT_SPLIT_MMA(FN)                                                                   \
+  for (int i = 0; i < 6; ++i) {                                                            \
+    if (i >= n) break;                                                                     \
+    const uint64_t a_ = adesc + (uint64_t)ao[i], b_ = bdesc + (uint64_t)(nstack ? ao[i] : bo[i]); \
+    FN(acc, a_, b_, i == 0 ? (first ^ 1u) : 1u);                                           \
+  }
+  if constexpr (NW == 32) {
+    if (fmt) { VT_SPLIT_MMA(wgmma_f16_n32) } else { VT_SPLIT_MMA(wgmma_bf16_n32) }
+  } else if constexpr (NW == 64) {
+    if (fmt) { VT_SPLIT_MMA(wgmma_f16_n64) } else { VT_SPLIT_MMA(wgmma_bf16_n64) }
+  } else {
+    if (fmt) { VT_SPLIT_MMA(wgmma_f16_n128) } else { VT_SPLIT_MMA(wgmma_bf16_n128) }
+  }
+#undef VT_SPLIT_MMA
+}
 
-template <int CG>
+template <int NW>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcArgs p) {
+  constexpr int MTMAX = (MAX_ACC_COLS / NW) < 4 ? (MAX_ACC_COLS / NW) : 4;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base;
   const uint32_t b_base = a_base + (uint32_t)p.a_stages * p.a_stage_bytes;
-  const uint32_t st_base = b_base + (uint32_t)p.b_stages * p.b_stage_bytes;
-  const uint32_t bar_base = st_base + 2 * STAGING_BYTES;
-  // barriers: a_full[8] a_empty[8] b_full[8] b_empty[8] tmem_full[2] tmem_empty[2]
+  const uint32_t bar_base = b_base + (uint32_t)p.b_stages * p.b_stage_bytes;
+  // barriers: a_full[8] a_empty[8] b_full[8] b_empty[8] a_ready[8]
   auto a_full = [&](int i) { return bar_base + 8u * i; };
   auto a_empty = [&](int i) { return bar_base + 64u + 8u * i; };
   auto b_full = [&](int i) { return bar_base + 128u + 8u * i; };
   auto b_empty = [&](int i) { return bar_base + 192u + 8u * i; };
-  auto t_full = [&](int i) { return bar_base + 256u + 8u * i; };
-  auto t_empty = [&](int i) { return bar_base + 272u + 8u * i; };
-  const uint32_t tmem_slot = bar_base + 288u;
-  auto a_ready = [&](int i) { return bar_base + 320u + 8u * i; };   // bf16x3: A stage converted to [hi|lo] bf16 rows
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
+  auto a_ready = [&](int i) { return bar_base + 256u + 8u * i; };   // bf16x3: A stage converted to [hi|lo] 16-bit rows
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;      // CTA rank in the pair
-  const int cta_i = (CG == 2) ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int cta_n = (CG == 2) ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  long long tw[4] = {0, 0, 0, 0};
-  const long long t_begin = clock64();
+  const int wg = threadIdx.x >> 7;
 
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < p.n_src; ++s)
       for (int v = 0; v < 4; ++v) tma_prefetch_desc(&p.in_map[s][v]);
     tma_prefetch_desc(&p.w_map);
-    for (int ph = 0; ph < p.n_phase; ++ph) tma_prefetch_desc(&p.out_map[ph]);
   }
   if (warp == 1 && lane == 0) {
-    for (int i = 0; i < p.a_stages; ++i) { mbar_init(a_full(i), 1); mbar_init(a_empty(i), 1); mbar_init(a_ready(i), XFORM_WARPS * CG); }
-    for (int i = 0; i < p.b_stages; ++i) { mbar_init(b_full(i), 1); mbar_init(b_empty(i), 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(t_full(i), 1); mbar_init(t_empty(i), 4 * CG); }
+    for (int i = 0; i < p.a_stages; ++i) { mbar_init(a_full(i), 1); mbar_init(a_empty(i), RELEASE_ARRIVALS); mbar_init(a_ready(i), XFORM_WARPS); }
+    for (int i = 0; i < p.b_stages; ++i) { mbar_init(b_full(i), 1); mbar_init(b_empty(i), RELEASE_ARRIVALS); }
     fence_barrier_init();
     fence_proxy_async_smem();
   }
-  if (warp == 2) {
-    if (CG == 2) tmem_alloc_2sm(tmem_slot, (uint32_t)p.tmem_cols);
-    else tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    tc_fence_before();
-  }
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
+  __syncthreads();
 
   const int m_tiles = p.B * p.tiles_y * p.tiles_x;
   const int tiles_per_img = p.tiles_y * p.tiles_x;
-  // a work item covers item_w x item_h output pixels (of the CTA pair if CG == 2; the pair is side by side or stacked)
-  const int item_w = TILE_W * p.mt * ((CG == 2 && !p.pair_y) ? 2 : 1);
-  const int item_h = TILE_H * ((CG == 2 && p.pair_y) ? 2 : 1);
-  const int rank_x = p.pair_y ? 0 : (int)rank * TILE_W * p.mt;   // this CTA's offset inside the work item
-  const int rank_y = p.pair_y ? (int)rank * TILE_H : 0;
+  const int item_w = TILE_W * p.mt;   // a work item covers item_w x TILE_H output pixels
 
-  if (warp == 0) {
-    // ================= TMA producer (whole warp converged; one elected lane issues) =================
-    // Issuing from a converged warp lets ptxas keep descriptors/coordinates in uniform registers; issuing from a
-    // `lane == 0` branch wraps every UTMALDG/UTCHMMA in an ELECT loop (measured 103 vs 59 cycles per MMA).
-    // ring positions are kept as (stage, parity) pairs and advanced incrementally: runtime-divisor % and / cost ~50-100
-    // cycles each on the issuing thread's critical path
-    int a_st = 0, b_st = 0;
-    uint32_t a_par = 0, b_par = 0;
-    for (int tile = cta_i; tile < p.total_tiles; tile += cta_n) {
-      const int n_tile = p.m_major ? tile % p.n_tiles : tile / m_tiles, m = p.m_major ? tile / p.n_tiles : tile % m_tiles;
-      const int b = m / tiles_per_img, rem = m % tiles_per_img;
-      const int oy0 = (rem / p.tiles_x) * item_h + rank_y, ox0 = (rem % p.tiles_x) * item_w + rank_x;
-      const int n0 = n_tile * p.block_n;
-      const int wb = p.wB > 1 ? b : 0;
-      for (int s = 0; s < p.n_src; ++s) {
-        for (int kc = 0; kc < p.kchunks[s]; ++kc) {
-          const int c0 = kc * KCH;
-          if (p.halo) {
-            VT_TWAIT(0, mbar_wait(a_empty(a_st), a_par ^ 1, 1));
-            if (elect_one()) {
-              const uint32_t st = a_base + a_st * p.a_stage_bytes;
-              if (CG == 2 && !p.bf16x3) {
-                if (rank == 0) mbar_arrive_expect_tx(a_full(a_st), 2u * (uint32_t)p.a_tx_bytes);
-                for (int v = 0; v < p.n_hv; ++v)
-                  tma_load_4d_2sm(st + p.hv_off[v], &p.in_map[s][p.hv_view[v]], a_full(a_st), c0, ox0 + p.hv_x0[v], oy0 + p.hv_y0[v], b);
-              } else {   // (bf16x3: every CTA's transform warps wait on their own a_full)
+  if (wg == 0) {
+    if (warp == 0) {
+      // ================= TMA producer (whole warp converged; one elected lane issues) =================
+      int a_st = 0, b_st = 0;
+      uint32_t a_par = 0, b_par = 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        const int n_tile = p.m_major ? tile % p.n_tiles : tile / m_tiles, m = p.m_major ? tile / p.n_tiles : tile % m_tiles;
+        const int b = m / tiles_per_img, rem = m % tiles_per_img;
+        const int oy0 = (rem / p.tiles_x) * TILE_H, ox0 = (rem % p.tiles_x) * item_w;
+        const int n0 = n_tile * p.block_n;
+        const int wb = p.wB > 1 ? b : 0;
+        for (int s = 0; s < p.n_src; ++s) {
+          for (int kc = 0; kc < p.kchunks[s]; ++kc) {
+            const int c0 = kc * KCH;
+            if (p.halo) {
+              mbar_wait(a_empty(a_st), a_par ^ 1);
+              if (elect_one()) {
+                const uint32_t st = a_base + a_st * p.a_stage_bytes;
                 mbar_arrive_expect_tx(a_full(a_st), (uint32_t)p.a_tx_bytes);
                 for (int v = 0; v < p.n_hv; ++v)
                   tma_load_4d(st + p.hv_off[v], &p.in_map[s][p.hv_view[v]], a_full(a_st), c0, ox0 + p.hv_x0[v], oy0 + p.hv_y0[v], b);
               }
-            }
-            __syncwarp();
-            if (++a_st == p.a_stages) { a_st = 0; a_par ^= 1; }
-          }
-          int gj = 0;   // position inside the current tap group
-          for (int j = 0; j < p.n_steps; ++j) {
-            if (!p.halo) {
-              VT_TWAIT(0, mbar_wait(a_empty(a_st), a_par ^ 1, 2));
-              if (elect_one()) {
-                mbar_arrive_expect_tx(a_full(a_st), (uint32_t)p.a_tx_bytes);
-                tma_load_4d(a_base + a_st * p.a_stage_bytes, &p.in_map[s][p.step_view[j]], a_full(a_st), c0, ox0 + p.step_vx[j],
-                            oy0 + p.step_vy[j], b);
-              }
               __syncwarp();
               if (++a_st == p.a_stages) { a_st = 0; a_par ^= 1; }
             }
-            if (gj == 0) {
-              // one TMA box carries the weight tiles of `tgroup` consecutive taps: (32 ch, block_n, tgroup, 1)
-              VT_TWAIT(1, mbar_wait(b_empty(b_st), b_par ^ 1, 3));
-              if (elect_one()) {
-                // bf16x3: the weight row of a 32-channel chunk is one 128-byte bf16 row [w_hi(32) | w_lo(32)]
-                const int wc = p.bf16x3 ? (p.coff[s] + c0) * 2 : p.coff[s] + c0;
-                if (CG == 2) {   // this CTA stages rows [rank*block_n/2, +block_n/2) of the weight tile
-                  if (rank == 0) mbar_arrive_expect_tx(b_full(b_st), 2u * (uint32_t)p.b_tx_bytes);
-                  tma_load_4d_2sm(b_base + b_st * p.b_stage_bytes, &p.w_map, b_full(b_st), wc,
-                                  (p.nstack ? 0 : n0) + (int)rank * (p.mma_n / 2), p.step_w[j], wb);
-                } else {
+            int gj = 0;   // position inside the current tap group
+            for (int j = 0; j < p.n_steps; ++j) {
+              if (!p.halo) {
+                mbar_wait(a_empty(a_st), a_par ^ 1);
+                if (elect_one()) {
+                  mbar_arrive_expect_tx(a_full(a_st), (uint32_t)p.a_tx_bytes);
+                  tma_load_4d(a_base + a_st * p.a_stage_bytes, &p.in_map[s][p.step_view[j]], a_full(a_st), c0, ox0 + p.step_vx[j],
+                              oy0 + p.step_vy[j], b);
+                }
+                __syncwarp();
+                if (++a_st == p.a_stages) { a_st = 0; a_par ^= 1; }
+              }
+              if (gj == 0) {
+                // one TMA box carries the weight tiles of `tgroup` consecutive taps: (32 ch, block_n, tgroup, 1)
+                mbar_wait(b_empty(b_st), b_par ^ 1);
+                if (elect_one()) {
+                  // bf16x3: the weight row of a 32-channel chunk is one 128-byte 16-bit row [w_hi(32) | w_lo(32)]
+                  const int wc = p.bf16x3 ? (p.coff[s] + c0) * 2 : p.coff[s] + c0;
                   mbar_arrive_expect_tx(b_full(b_st), (uint32_t)p.b_tx_bytes);
-                  tma_load_4d(b_base + b_st * p.b_stage_bytes, &p.w_map, b_full(b_st), wc, n0, p.step_w[j], wb);
+                  tma_load_4d(b_base + b_st * p.b_stage_bytes, &p.w_map, b_full(b_st), wc, p.nstack ? 0 : n0, p.step_w[j], wb);
+                }
+                __syncwarp();
+                if (++b_st == p.b_stages) { b_st = 0; b_par ^= 1; }
+              }
+              if (++gj == p.tgroup) gj = 0;
+            }
+          }
+        }
+      }
+    } else if (p.bf16x3) {
+      // ================= operand transform (bf16x3): fp32 rows -> [hi(32) | lo(32)] 16-bit rows, in place =================
+      // A 32-channel fp32 row (128 B) becomes the K = 64 row [a_hi | a_lo] with a_hi = bf16(a), a_lo = bf16(a - a_hi);
+      // 16-byte chunk j of the row lives at physical chunk j ^ ((addr >> 7) & 7) (SWIZZLE_128B as TMA wrote it, kept for the MMA).
+      const int t = (warp - 1) * 32 + lane;   // 0 .. 32 * XFORM_WARPS
+      const int rows = p.a_rows;
+      int a_st = 0;
+      uint32_t a_par = 0;
+      const int bw = p.halo ? p.halo_w : TILE_W;   // pixels per box row
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        const int m = p.m_major ? tile / p.n_tiles : tile % m_tiles;
+        const int b = m / tiles_per_img, rem = m % tiles_per_img;
+        const int oy0 = (rem / p.tiles_x) * TILE_H, ox0 = (rem % p.tiles_x) * item_w;
+        for (int s = 0; s < p.n_src; ++s) {
+          const float* sc = p.src_scale[s];
+          const float* aff = p.src_affine[s];
+          for (int kc = 0; kc < p.kchunks[s]; ++kc) {
+            const float4* affp = aff ? reinterpret_cast<const float4*>(aff + ((int64_t)b * p.src_cn[s] + kc * KCH) * 2) : nullptr;
+            const int loads = p.halo ? 1 : p.n_steps;
+            for (int l = 0; l < loads; ++l) {
+              mbar_wait(a_full(a_st), a_par);
+              const uint32_t stage = a_base + a_st * p.a_stage_bytes;
+              const int bx0 = ox0 + (p.halo ? p.halo_x0 : p.step_vx[l]), by0 = oy0 + (p.halo ? p.halo_y0 : p.step_vy[l]);
+              for (int r = t; r < rows; r += 32 * XFORM_WARPS) {
+                const uint32_t row = stage + (uint32_t)r * 128u;
+                const uint32_t ph = (row >> 7) & 7u;
+                float f[32];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                  float4 v;
+                  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(row + ((j ^ ph) << 4)));
+                  f[4 * j] = v.x; f[4 * j + 1] = v.y; f[4 * j + 2] = v.z; f[4 * j + 3] = v.w;
+                }
+                if (sc || aff) {   // rows are box pixels in raster order
+                  const int ry = r / bw, rx = r - ry * bw;
+                  const int ix = bx0 + rx, iy = by0 + ry;
+                  const bool inb = ix >= 0 && ix < p.in_w && iy >= 0 && iy < p.in_h;
+                  if (aff && inb) {   // per-(sample, channel) affine (AdaIN) on real pixels; the zero padding stays zero
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                      const float4 q = __ldg(affp + j);   // (scale, shift) of channels 2j, 2j+1 (same address in every thread)
+                      f[2 * j] = fmaf(f[2 * j], q.x, q.y);
+                      f[2 * j + 1] = fmaf(f[2 * j + 1], q.z, q.w);
+                    }
+                  }
+                  if (sc) {           // per-pixel multiplier of this source (f_E * m_E)
+                    const float mm = inb ? __ldg(sc + (int64_t)b * p.sc_sb + (int64_t)iy * p.sc_sy + (int64_t)ix * p.sc_sx) : 0.f;
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) f[i] *= mm;
+                  }
+                }
+                uint32_t hi[16], lo[16];
+                if (p.fmt) {
+#pragma unroll
+                  for (int i = 0; i < 16; ++i) split_f16x2(f[2 * i], f[2 * i + 1], hi[i], lo[i]);
+                } else {
+#pragma unroll
+                  for (int i = 0; i < 16; ++i) {
+                    // packed converts (one cvt.rn.bf16x2.f32 per pair); a bf16 widened to fp32 is its bits shifted left by 16
+                    const __nv_bfloat162 h2 = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
+                    hi[i] = *reinterpret_cast<const uint32_t*>(&h2);
+                    const float r0 = f[2 * i] - __uint_as_float(hi[i] << 16), r1 = f[2 * i + 1] - __uint_as_float(hi[i] & 0xffff0000u);
+                    const __nv_bfloat162 l2 = __floats2bfloat162_rn(r0, r1);
+                    lo[i] = *reinterpret_cast<const uint32_t*>(&l2);
+                  }
+                }
+#pragma unroll
+                for (int m4 = 0; m4 < 4; ++m4) {
+                  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row + ((m4 ^ ph) << 4)), "r"(hi[4 * m4]), "r"(hi[4 * m4 + 1]), "r"(hi[4 * m4 + 2]), "r"(hi[4 * m4 + 3]) : "memory");
+                  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row + (((m4 + 4) ^ ph) << 4)), "r"(lo[4 * m4]), "r"(lo[4 * m4 + 1]), "r"(lo[4 * m4 + 2]), "r"(lo[4 * m4 + 3]) : "memory");
                 }
               }
+              // generic-proxy writes -> visible to the tensor core's async-proxy reads
+              fence_proxy_async_smem();
               __syncwarp();
-              if (++b_st == p.b_stages) { b_st = 0; b_par ^= 1; }
+              if (lane == 0) mbar_arrive(a_ready(a_st));
+              if (++a_st == p.a_stages) { a_st = 0; a_par ^= 1; }
             }
-            if (++gj == p.tgroup) gj = 0;
           }
         }
       }
     }
-  } else if (warp == 1 && rank == 0) {
-    // ================= MMA issuer (whole warp converged; one elected lane issues; CTA rank 0 only) =================
-    const uint32_t idesc = p.bf16x3 ? (p.fmt ? make_idesc_f16(TILE_M * CG, p.mma_n) : make_idesc_bf16(TILE_M * CG, p.mma_n))
-                                    : make_idesc_tf32(TILE_M * CG, p.mma_n);
-    int a_st = 0, b_st = 0, as = 0;
-    uint32_t a_par = 0, b_par = 0, t_par = 0;
-    const uint32_t tile_bytes_n = (uint32_t)(p.mma_n / CG) * 128u;   // bytes of one tap's weight rows held by this CTA
-    for (int tile = cta_i; tile < p.total_tiles; tile += cta_n) {
-      VT_TWAIT(2, mbar_wait(t_empty(as), t_par ^ 1, 4));
-      tc_fence_after();
-      const uint32_t d_tmem0 = tmem_base + (uint32_t)(as * p.mt * p.mma_n);
+  } else {
+    // ================= consumers: wgmma main loop + epilogue =================
+    const int c = wg - 1;                       // pixel rows [8c, 8c + 8) of the 8 x 16 tile
+    const int tw_ = (threadIdx.x & 127) >> 5;   // warp inside the warpgroup: accumulator rows [16 tw_, 16 tw_ + 16)
+    const bool leader = lane == 0;   // one arrival per consumer warp
+    const int qd = lane & 3;                    // column pair inside each 8-column group
+    float acc[MTMAX][NW / 2];
+#pragma unroll
+    for (int g = 0; g < MTMAX; ++g)
+#pragma unroll
+      for (int i = 0; i < NW / 2; ++i) acc[g][i] = 0.f;
+    const float nw = (p.noise && p.noise_w) ? *p.noise_w : 0.f;
+    int a_st = 0, b_st = 0;
+    uint32_t a_par = 0, b_par = 0;
+    const uint32_t tile_bytes_n = (uint32_t)p.mma_n * 128u;   // bytes of one tap's weight rows
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const int n_tile = p.m_major ? tile % p.n_tiles : tile / m_tiles, m = p.m_major ? tile / p.n_tiles : tile % m_tiles;
+      const int b = m / tiles_per_img, rem = m % tiles_per_img;
+      const int oy0 = (rem / p.tiles_x) * TILE_H, ox0 = (rem % p.tiles_x) * item_w;
+      const int n0 = n_tile * p.block_n;
       uint32_t first = 1;   // first K step of this work item overwrites the accumulators
+      int rel_a = -1, rel_b = -1;   // stages the previous (still in flight) wgmma group reads, released once it has completed
       for (int s = 0; s < p.n_src; ++s) {
         for (int kc = 0; kc < p.kchunks[s]; ++kc) {
-          if (p.halo) {
-            VT_TWAIT(0, mbar_wait(p.bf16x3 ? a_ready(a_st) : a_full(a_st), a_par, 5));
-          }
+          if (p.halo) mbar_wait(p.bf16x3 ? a_ready(a_st) : a_full(a_st), a_par);
           int gj = 0;
           for (int j = 0; j < p.n_steps; ++j) {
-            if (!p.halo) {
-              VT_TWAIT(0, mbar_wait(p.bf16x3 ? a_ready(a_st) : a_full(a_st), a_par, 6));
-            }
-            if (gj == 0) {
-              VT_TWAIT(1, mbar_wait(b_full(b_st), b_par, 7));
-            }
-            tc_fence_after();
+            if (!p.halo) mbar_wait(p.bf16x3 ? a_ready(a_st) : a_full(a_st), a_par);
+            if (gj == 0) mbar_wait(b_full(b_st), b_par);
             uint32_t a_addr = a_base + a_st * p.a_stage_bytes;
             uint32_t sbo = 1024;
             if (p.halo) {
-              // The 128B swizzle is a function of the absolute smem address bits (TMA wrote the halo box with the
-              // same function), so a tap is just a start address shifted by whole 128-byte rows; the descriptor's
-              // base-offset field stays 0 (setting it to (addr>>7)&7 was measured WRONG on B200, see DESIGN.md).
+              // the 128B swizzle follows the absolute smem address bits (TMA wrote the halo box with the same function), so a
+              // tap is just a start address shifted by whole 128-byte rows
               a_addr += (uint32_t)p.step_aoff[j];
               sbo = (uint32_t)p.step_sbo[j];
             }
-            const uint64_t bdesc = make_smem_desc_sw128(b_base + b_st * p.b_stage_bytes + (uint32_t)gj * tile_bytes_n, 1024, 0);
+            a_addr += 8u * (uint32_t)c * sbo;   // this warpgroup's 8 pixel rows = 8 row groups of 8 pixels
+            const uint64_t bdesc = make_smem_desc_sw128(b_base + b_st * p.b_stage_bytes + (uint32_t)gj * tile_bytes_n, 1024);
             const bool last_of_group = (gj == p.tgroup - 1);
-            if (elect_one()) {
-              for (int g = 0; g < p.mt; ++g) {
-                const uint64_t adesc = make_smem_desc_sw128(a_addr + (uint32_t)(g * TILE_W * 128), sbo, 0);
-                const uint32_t d_tmem = d_tmem0 + (uint32_t)(g * p.mma_n);
-                if (p.nstack) {
-                  // [a_hi|a_lo] (K = 64) x rows [w_hi|w_hi] (columns 0..31) and [w_lo|w_lo] (columns 32..63): all four products,
-                  // 4 instructions per tap instead of 6; the epilogue adds the two column halves
-                  if (CG == 2) {
-                    umma_bf16_2sm(d_tmem, adesc, bdesc, idesc, first ^ 1u);
-                    umma_bf16_2sm(d_tmem, adesc + 2, bdesc + 2, idesc, 1);
-                    umma_bf16_2sm(d_tmem, adesc + 4, bdesc + 4, idesc, 1);
-                    umma_bf16_2sm(d_tmem, adesc + 6, bdesc + 6, idesc, 1);
-                  } else {
-                    umma_bf16(d_tmem, adesc, bdesc, idesc, first ^ 1u);
-                    umma_bf16(d_tmem, adesc + 2, bdesc + 2, idesc, 1);
-                    umma_bf16(d_tmem, adesc + 4, bdesc + 4, idesc, 1);
-                    umma_bf16(d_tmem, adesc + 6, bdesc + 6, idesc, 1);
-                  }
-                } else if (p.bf16x3) {
-                  // a*w ~= a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the dropped a_lo*w_lo term is ~2^-18 relative). The A row is
-                  // [a_hi(32)|a_lo(32)] and the B row [w_hi(32)|w_lo(32)] bf16; +2 on a descriptor = +32 B = 16 bf16 of K.
-                  if (CG == 2) {
-                    umma_bf16_2sm(d_tmem, adesc, bdesc, idesc, first ^ 1u);
-                    umma_bf16_2sm(d_tmem, adesc + 2, bdesc + 2, idesc, 1);
-                    umma_bf16_2sm(d_tmem, adesc + 4, bdesc, idesc, 1);
-                    umma_bf16_2sm(d_tmem, adesc + 6, bdesc + 2, idesc, 1);
-                    umma_bf16_2sm(d_tmem, adesc, bdesc + 4, idesc, 1);
-                    umma_bf16_2sm(d_tmem, adesc + 2, bdesc + 6, idesc, 1);
-                  } else {
-                    umma_bf16(d_tmem, adesc, bdesc, idesc, first ^ 1u);
-                    umma_bf16(d_tmem, adesc + 2, bdesc + 2, idesc, 1);
-                    umma_bf16(d_tmem, adesc + 4, bdesc, idesc, 1);
-                    umma_bf16(d_tmem, adesc + 6, bdesc + 2, idesc, 1);
-                    umma_bf16(d_tmem, adesc, bdesc + 4, idesc, 1);
-                    umma_bf16(d_tmem, adesc + 2, bdesc + 6, idesc, 1);
-                  }
-                } else if (CG == 2) {
-                  umma_tf32_2sm(d_tmem, adesc, bdesc, idesc, first ^ 1u);
-                  umma_tf32_2sm(d_tmem, adesc + 2, bdesc + 2, idesc, 1);
-                  umma_tf32_2sm(d_tmem, adesc + 4, bdesc + 4, idesc, 1);
-                  umma_tf32_2sm(d_tmem, adesc + 6, bdesc + 6, idesc, 1);
-                } else {
-                  umma_tf32(d_tmem, adesc, bdesc, idesc, first ^ 1u);
-                  umma_tf32(d_tmem, adesc + 2, bdesc + 2, idesc, 1);
-                  umma_tf32(d_tmem, adesc + 4, bdesc + 4, idesc, 1);
-                  umma_tf32(d_tmem, adesc + 6, bdesc + 6, idesc, 1);
-                }
+            wgmma_fence();
+#pragma unroll
+            for (int g = 0; g < MTMAX; ++g) {
+              if (g < p.mt) {
+                const uint64_t adesc = make_smem_desc_sw128(a_addr + (uint32_t)(g * TILE_W * 128), sbo);
+                mma_step<NW>(acc[g], adesc, bdesc, first, p.bf16x3, p.fmt, p.nstack);
               }
-              if (last_of_group) { if (CG == 2) umma_commit_2sm(b_empty(b_st)); else umma_commit(b_empty(b_st)); }
-              if (!p.halo) { if (CG == 2) umma_commit_2sm(a_empty(a_st)); else umma_commit(a_empty(a_st)); }
             }
-            __syncwarp();
+            wgmma_commit();
+            wgmma_wait<1>();   // this warp's share of the group before this one has completed: its stages may be refilled
+            if (leader) {
+              if (rel_a >= 0) mbar_arrive(a_empty(rel_a));
+              if (rel_b >= 0) mbar_arrive(b_empty(rel_b));
+            }
+            rel_a = (!p.halo || j == p.n_steps - 1) ? a_st : -1;
+            rel_b = last_of_group ? b_st : -1;
             first = 0;
             if (last_of_group) { gj = 0; if (++b_st == p.b_stages) { b_st = 0; b_par ^= 1; } } else { ++gj; }
-            if (!p.halo) { if (++a_st == p.a_stages) { a_st = 0; a_par ^= 1; } }
-          }
-          if (p.halo) {
-            if (elect_one()) { if (CG == 2) umma_commit_2sm(a_empty(a_st)); else umma_commit(a_empty(a_st)); }
-            __syncwarp();
-            if (++a_st == p.a_stages) { a_st = 0; a_par ^= 1; }
+            if (!p.halo || j == p.n_steps - 1) { if (++a_st == p.a_stages) { a_st = 0; a_par ^= 1; } }
           }
         }
       }
-      if (elect_one()) { if (CG == 2) umma_commit_2sm(t_full(as)); else umma_commit(t_full(as)); }
-      __syncwarp();
-      if (++as == p.acc_stages) { as = 0; t_par ^= 1; }
-    }
-  } else if ((warp == 2 || warp == 3 || warp >= 8) && p.bf16x3) {
-    // ================= operand transform (bf16x3): fp32 rows -> [hi(32) | lo(32)] bf16 rows, in place =================
-    // A 32-channel fp32 row (128 B) becomes the K = 64 bf16 row [a_hi | a_lo] with a_hi = bf16(a), a_lo = bf16(a - a_hi);
-    // 16-byte chunk j of the row lives at physical chunk j ^ ((addr >> 7) & 7) (SWIZZLE_128B as TMA wrote it, kept for the MMA).
-    const int t = (warp < 4 ? warp - 2 : warp - 6) * 32 + lane;   // 0 .. 32 * XFORM_WARPS
-    const int rows = p.a_rows;
-    int a_st = 0;
-    uint32_t a_par = 0;
-    const int bw = p.halo ? p.halo_w : TILE_W;   // pixels per box row
-    for (int tile = cta_i; tile < p.total_tiles; tile += cta_n) {
-      const int m = p.m_major ? tile / p.n_tiles : tile % m_tiles;
-      const int b = m / tiles_per_img, rem = m % tiles_per_img;
-      const int oy0 = (rem / p.tiles_x) * item_h + rank_y, ox0 = (rem % p.tiles_x) * item_w + rank_x;
-      for (int s = 0; s < p.n_src; ++s) {
-        const float* sc = p.src_scale[s];
-        const float* aff = p.src_affine[s];
-        for (int kc = 0; kc < p.kchunks[s]; ++kc) {
-          const float4* affp = aff ? reinterpret_cast<const float4*>(aff + ((int64_t)b * p.src_cn[s] + kc * KCH) * 2) : nullptr;
-          const int loads = p.halo ? 1 : p.n_steps;
-          for (int l = 0; l < loads; ++l) {
-            VT_TWAIT(0, mbar_wait(a_full(a_st), a_par, 9));
-            const uint32_t stage = a_base + a_st * p.a_stage_bytes;
-            const int bx0 = ox0 + (p.halo ? p.halo_x0 : p.step_vx[l]), by0 = oy0 + (p.halo ? p.halo_y0 : p.step_vy[l]);
-            for (int r = t; r < rows; r += 32 * XFORM_WARPS) {
-              const uint32_t row = stage + (uint32_t)r * 128u;
-              const uint32_t ph = (row >> 7) & 7u;
-              float f[32];
+      wgmma_wait<0>();
 #pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                float4 v;
-                asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(row + ((j ^ ph) << 4)));
-                f[4 * j] = v.x; f[4 * j + 1] = v.y; f[4 * j + 2] = v.z; f[4 * j + 3] = v.w;
-              }
-              if (sc || aff) {   // rows are box pixels in raster order
-                const int ry = r / bw, rx = r - ry * bw;
-                const int ix = bx0 + rx, iy = by0 + ry;
-                const bool inb = ix >= 0 && ix < p.in_w && iy >= 0 && iy < p.in_h;
-                if (aff && inb) {   // per-(sample, channel) affine (AdaIN) on real pixels; the zero padding stays zero
-#pragma unroll
-                  for (int j = 0; j < 16; ++j) {
-                    const float4 q = __ldg(affp + j);   // (scale, shift) of channels 2j, 2j+1 (same address in every thread)
-                    f[2 * j] = fmaf(f[2 * j], q.x, q.y);
-                    f[2 * j + 1] = fmaf(f[2 * j + 1], q.z, q.w);
-                  }
-                }
-                if (sc) {           // per-pixel multiplier of this source (f_E * m_E)
-                  const float mm = inb ? __ldg(sc + (int64_t)b * p.sc_sb + (int64_t)iy * p.sc_sy + (int64_t)ix * p.sc_sx) : 0.f;
-#pragma unroll
-                  for (int i = 0; i < 32; ++i) f[i] *= mm;
-                }
-              }
-              uint32_t hi[16], lo[16];
-              if (p.fmt) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) split_f16x2(f[2 * i], f[2 * i + 1], hi[i], lo[i]);
-              } else {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                  // packed converts (one cvt.rn.bf16x2.f32 per pair); a bf16 widened to fp32 is its bits shifted left by 16
-                  const __nv_bfloat162 h2 = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-                  hi[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                  const float r0 = f[2 * i] - __uint_as_float(hi[i] << 16), r1 = f[2 * i + 1] - __uint_as_float(hi[i] & 0xffff0000u);
-                  const __nv_bfloat162 l2 = __floats2bfloat162_rn(r0, r1);
-                  lo[i] = *reinterpret_cast<const uint32_t*>(&l2);
-                }
-              }
-#pragma unroll
-              for (int m4 = 0; m4 < 4; ++m4) {
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row + ((m4 ^ ph) << 4)), "r"(hi[4 * m4]), "r"(hi[4 * m4 + 1]), "r"(hi[4 * m4 + 2]), "r"(hi[4 * m4 + 3]) : "memory");
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row + (((m4 + 4) ^ ph) << 4)), "r"(lo[4 * m4]), "r"(lo[4 * m4 + 1]), "r"(lo[4 * m4 + 2]), "r"(lo[4 * m4 + 3]) : "memory");
-              }
-            }
-            // generic-proxy writes -> visible to the tensor core's async-proxy reads.  The fence also waits until every lane's stores
-            // are performed in this SM's shared memory (one copy, no cache), so the pair's issuing thread only needs a plain remote
-            // arrive; a cluster-scope release compiles to MEMBAR.ALL.GPU (~2k cycles per stage, measured in conv_rs.cu)
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) { if (CG == 2) { if (p.strict_release) mbar_arrive_cta0_release(a_ready(a_st)); else mbar_arrive_cta0(a_ready(a_st)); } else mbar_arrive(a_ready(a_st)); }
-            if (++a_st == p.a_stages) { a_st = 0; a_par ^= 1; }
-          }
-        }
+      for (int g = 0; g < MTMAX; ++g) wgmma_pin<NW / 2>(acc[g]);
+      if (leader) {
+        if (rel_a >= 0) mbar_arrive(a_empty(rel_a));
+        if (rel_b >= 0) mbar_arrive(b_empty(rel_b));
       }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ================= epilogue =================
-    const int q = warp - 4;
-    const int r = q * 32 + lane;           // accumulator row == pixel index in the M tile
-    const int ty = r / TILE_W, tx = r % TILE_W;
-    const bool store_thread = (threadIdx.x == 128);
-    const float nw = (p.noise && p.noise_w) ? *p.noise_w : 0.f;
-    uint32_t chunk = 0;
-    const int nchunks = p.block_n / 32;
-    int as = 0;
-    uint32_t t_par = 0;
-    for (int tile = cta_i; tile < p.total_tiles; tile += cta_n) {
-      const int n_tile = p.m_major ? tile % p.n_tiles : tile / m_tiles, m = p.m_major ? tile / p.n_tiles : tile % m_tiles;
-      const int b = m / tiles_per_img, rem = m % tiles_per_img;
-      const int oy0 = (rem / p.tiles_x) * item_h + rank_y, ox0 = (rem % p.tiles_x) * item_w + rank_x;
-      const int n0 = n_tile * p.block_n;
-      // single-phase layers: fetch this thread's noise values before waiting for the accumulators (an exposed HBM latency per
-      // tile otherwise; the noise map is streamed once)
-      float nz_pre[4] = {0.f, 0.f, 0.f, 0.f};
-      if (p.noise && p.n_phase == 1) {
+
+      // ---- epilogue. Accumulator register i of a thread holds row 16 tw_ + lane/4 + 8 ((i/2)%2) (a pixel of the tile) and
+      // column 8 (i/4) + 2 qd + (i%2): every thread owns two pixels (same x, rows ty and ty + 1) and 2-channel pairs of them.
+      const int r0 = 64 * c + 16 * tw_ + (lane >> 2);
+      const int ty = r0 / TILE_W, tx = r0 % TILE_W;   // second pixel: ty + 1
+      const int ph0 = n0 / p.Cout, nb0 = n0 - ph0 * p.Cout;
+      const int nchunks = p.block_n / 32;
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int oy = oy0 + ty, ox = ox0 + g * TILE_W + tx;
-          if (g < p.mt && oy < p.Ho && ox < p.Wo)
-            nz_pre[g] = nw * __ldg(p.noise + p.phase_pix[0] + (int64_t)b * p.pix_sb + (int64_t)oy * p.pix_sy + (int64_t)ox * p.pix_sx);
+      for (int g = 0; g < MTMAX; ++g) {
+        if (g >= p.mt) break;
+        int oy[2], ox[2];
+        bool in_img[2];
+        int64_t off0[2], pix0[2];
+        float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          oy[h] = oy0 + ty + h; ox[h] = ox0 + g * TILE_W + tx;
+          in_img[h] = oy[h] < p.Ho && ox[h] < p.Wo;
+          off0[h] = (int64_t)b * p.out_sb + (int64_t)oy[h] * p.out_sy + (int64_t)ox[h] * p.out_sx;
+          pix0[h] = (int64_t)b * p.pix_sb + (int64_t)oy[h] * p.pix_sy + (int64_t)ox[h] * p.pix_sx;   // dense-pixel index
         }
-      }
-      VT_TWAIT(0, mbar_wait(t_full(as), t_par, 8));
-      tc_fence_after();
-      const int ph0 = n0 / p.Cout, nb0 = n0 - ph0 * p.Cout;   // once per work item
-      for (int g = 0; g < p.mt; ++g) {
-        const int oy = oy0 + ty, ox = ox0 + g * TILE_W + tx;
-        const bool in_img = oy < p.Ho && ox < p.Wo;
-        const int64_t off0 = (int64_t)b * p.out_sb + (int64_t)oy * p.out_sy + (int64_t)ox * p.out_sx;
-        const int64_t pix0 = (int64_t)b * p.pix_sb + (int64_t)oy * p.pix_sy + (int64_t)ox * p.pix_sx;   // dense-pixel index
-        float rgb0 = 0.f, rgb1 = 0.f, rgb2 = 0.f;   // fused ToRGB partial sums of this thread's pixel
         int ph = ph0, nb = nb0 - 32;
-        for (int j = 0; j < nchunks; ++j, ++chunk) {
+#pragma unroll
+        for (int j = 0; j < NW / 32; ++j) {
+          if (j >= nchunks) break;
           // column -> (phase, channel): the N dimension is phase-major [n_phase][Cout]; a 32-column chunk never straddles
           nb += 32;
           if (nb >= p.Cout) { nb -= p.Cout; ++ph; }
-          const int64_t off = p.phase_off[ph] + off0;
-          const float nz = p.n_phase == 1 ? nz_pre[g] : ((p.noise && in_img) ? nw * p.noise[p.phase_pix[ph] + pix0] : 0.f);
-          float v[32];
-          VT_TWAIT(1, tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((as * p.mt + g) * p.mma_n + j * 32), v));
-          if (p.nstack) {   // second column half: the w_lo products
-            float v2[32];
-            tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((as * p.mt + g) * p.mma_n + 32), v2);
+          float nz[2];
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] += v2[i];
-          }
-          if (p.acc_scale != 1.f) {
+          for (int h = 0; h < 2; ++h) nz[h] = (p.noise && in_img[h]) ? nw * __ldg(p.noise + p.phase_pix[ph] + pix0[h]) : 0.f;
+          // v[h][k][e]: pixel h, channel nb + 8k + 2qd + e
+          float v[2][4][2];
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] *= p.acc_scale;
-          }
-          const long long t_math0 = p.dbg ? clock64() : 0;
-          if (g == p.mt - 1 && j == nchunks - 1) {
-            // every accumulator of this stage is in registers: hand the TMEM stage back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { if (CG == 2) mbar_arrive_cta0(t_empty(as)); else mbar_arrive(t_empty(as)); }
-          }
-          // straight-line math: the 32 bias values come in as 8 vector loads issued together (a per-element __ldg inside a
-          // branchy loop serialised 32 L1 latencies: ~4k cycles per chunk, measured), and the activation is selected
-          // outside the element loop
-          if (p.bias) {
-            const float4* bp = reinterpret_cast<const float4*>(p.bias + nb);
-            float4 bq[8];
+          for (int k = 0; k < 4; ++k)
 #pragma unroll
-            for (int i = 0; i < 8; ++i) bq[i] = __ldg(bp + i);
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              v[4 * i + 0] += bq[i].x; v[4 * i + 1] += bq[i].y; v[4 * i + 2] += bq[i].z; v[4 * i + 3] += bq[i].w;
-            }
-          }
-          if (p.noise) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] += nz;
-          }
-          if (p.act == VT_ACT_LRELU) {
-            if (p.slope_vec) {   // PReLU: per-channel negative slope
-              const float4* sp = reinterpret_cast<const float4*>(p.slope_vec + nb);
-              float4 sq[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) sq[i] = __ldg(sp + i);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                v[4 * i + 0] = vt_lrelu(v[4 * i + 0], sq[i].x) * p.gain; v[4 * i + 1] = vt_lrelu(v[4 * i + 1], sq[i].y) * p.gain;
-                v[4 * i + 2] = vt_lrelu(v[4 * i + 2], sq[i].z) * p.gain; v[4 * i + 3] = vt_lrelu(v[4 * i + 3], sq[i].w) * p.gain;
+              for (int e = 0; e < 2; ++e) {
+                const int i = 16 * j + 4 * k + 2 * h + e;
+                float x = acc[g][i];
+                if (NW == 64 && p.nstack) x += acc[g][(i + 16) % (NW / 2)];   // second column half: the w_lo products
+                v[h][k][e] = x * p.acc_scale;
               }
-            } else {
 #pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = vt_lrelu(v[i], p.slope) * p.gain;
-            }
-          } else if (p.act == VT_ACT_RELU_TANH) {
+          for (int k = 0; k < 4; ++k) {
+            const int ch = nb + 8 * k + 2 * qd;
+            float2 bq = make_float2(0.f, 0.f), sq = make_float2(p.slope, p.slope);
+            if (p.bias) bq = __ldg(reinterpret_cast<const float2*>(p.bias + ch));
+            if (p.slope_vec) sq = __ldg(reinterpret_cast<const float2*>(p.slope_vec + ch));
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = tanhf(fmaxf(v[i], 0.f));
-          }
-          if (p.res) {
-            if (in_img) {
-              const float4* rp = reinterpret_cast<const float4*>(p.res + off + nb);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 rv = __ldg(rp + i);
-                v[4 * i + 0] = v[4 * i + 0] * p.alpha + p.beta * rv.x;
-                v[4 * i + 1] = v[4 * i + 1] * p.alpha + p.beta * rv.y;
-                v[4 * i + 2] = v[4 * i + 2] * p.alpha + p.beta * rv.z;
-                v[4 * i + 3] = v[4 * i + 3] * p.alpha + p.beta * rv.w;
+            for (int h = 0; h < 2; ++h) {
+              float v0 = v[h][k][0] + bq.x + nz[h], v1 = v[h][k][1] + bq.y + nz[h];
+              if (p.act == VT_ACT_LRELU) {
+                v0 = vt_lrelu(v0, sq.x) * p.gain; v1 = vt_lrelu(v1, sq.y) * p.gain;
+              } else if (p.act == VT_ACT_RELU_TANH) {
+                v0 = tanhf(fmaxf(v0, 0.f)); v1 = tanhf(fmaxf(v1, 0.f));
               }
-            }
-          } else if (p.alpha != 1.f) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] *= p.alpha;
-          }
-          if (p.round_tf32) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = vt_round_tf32(v[i]);
-          }
-          if (p.dbg) tw[2] += clock64() - t_math0;
-          const long long t_st0 = p.dbg ? clock64() : 0;
-          if (p.rgb_w) {
-            // 1x1 modulated conv to 3 channels on the values just produced (model/stylegan/model.py:384-385)
-            const float4* w0 = reinterpret_cast<const float4*>(p.rgb_w + ((int64_t)(p.wB > 1 ? b : 0) * 3) * p.Cout + nb);
-            const float4* w1 = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(w0) + p.Cout);
-            const float4* w2 = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(w0) + 2 * p.Cout);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float4 a0 = __ldg(w0 + i), a1 = __ldg(w1 + i), a2 = __ldg(w2 + i);
-              rgb0 = fmaf(v[4 * i], a0.x, rgb0); rgb0 = fmaf(v[4 * i + 1], a0.y, rgb0); rgb0 = fmaf(v[4 * i + 2], a0.z, rgb0); rgb0 = fmaf(v[4 * i + 3], a0.w, rgb0);
-              rgb1 = fmaf(v[4 * i], a1.x, rgb1); rgb1 = fmaf(v[4 * i + 1], a1.y, rgb1); rgb1 = fmaf(v[4 * i + 2], a1.z, rgb1); rgb1 = fmaf(v[4 * i + 3], a1.w, rgb1);
-              rgb2 = fmaf(v[4 * i], a2.x, rgb2); rgb2 = fmaf(v[4 * i + 1], a2.y, rgb2); rgb2 = fmaf(v[4 * i + 2], a2.z, rgb2); rgb2 = fmaf(v[4 * i + 3], a2.w, rgb2);
-            }
-          }
-          if (p.direct_store) {
-            // each thread owns one pixel's 32-channel run = one full 128-byte line of the NHWC output: no staging, no barriers
-            if (in_img) {
-              float4* op = reinterpret_cast<float4*>(p.out + off + nb);
-#pragma unroll
-              for (int c = 0; c < 8; ++c) op[c] = make_float4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-            }
-          } else {
-          const uint32_t sbuf = st_base + (chunk & 1) * STAGING_BYTES;
-          if (p.warp_store) {
-            // per-warp form: the warp's 32 pixels are rows 4q .. 4q+3 of the tile = a 4 KB slice of the staging buffer (a whole
-            // number of 1 KB swizzle atoms), stored through the same map with a box of 4 rows.  No CTA-wide barrier: a warp that
-            // is ahead starts its next chunk instead of waiting for the slowest one twice per chunk.
-            if (lane == 0) tma_store_wait_read<1>();    // this warp's store of two chunks ago has read the slice
-            __syncwarp();
-          } else {
-            if (store_thread) tma_store_wait_read<1>();   // the store that used this buffer two chunks ago has read it
-            named_bar_sync(1, 128);
-          }
-          const uint32_t row = sbuf + (uint32_t)r * 128u;
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const uint32_t dst = row + (uint32_t)((c ^ (r & 7)) << 4);
-            asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "f"(v[4 * c]), "f"(v[4 * c + 1]),
-                         "f"(v[4 * c + 2]), "f"(v[4 * c + 3])
-                         : "memory");
-          }
-          fence_proxy_async_smem();
-          if (p.warp_store) {
-            __syncwarp();
-            if (lane == 0) {
-              tma_store_4d(&p.out_map[ph], sbuf + (uint32_t)q * 4096u, nb, ox0 + g * TILE_W, oy0 + q * 4, b);
-              tma_store_commit();
-            }
-            if (p.stats_ws) {
-              // AdaptiveInstanceNorm statistics of the tensor this launch writes (model/dualstylegan.py:10-21), taken from the staged
-              // values: lane c adds channel nb + c over the warp's 32 pixels in row order (fixed order, no atomics), rows outside
-              // the image masked.  Word c of row rr sits in 16-byte chunk (c / 4) ^ (rr & 7): 32 distinct banks per read.
-              const unsigned okm = __ballot_sync(0xffffffffu, in_img);
-              float ssum = 0.f, ssq = 0.f;
-              const uint32_t wbase = sbuf + (uint32_t)q * 4096u + (uint32_t)((lane & 3) << 2);
-#pragma unroll 8
-              for (int rr = 0; rr < 32; ++rr) {
-                float xv;
-                asm volatile("ld.shared.f32 %0, [%1];" : "=f"(xv) : "r"(wbase + (uint32_t)rr * 128u + (uint32_t)((((lane >> 2) ^ (rr & 7))) << 4)));
-                if ((okm >> rr) & 1u) { ssum += xv; ssq = fmaf(xv, xv, ssq); }
+              const int64_t off = p.phase_off[ph] + off0[h] + ch;
+              if (p.res) {
+                if (in_img[h]) {
+                  const float2 rv = __ldg(reinterpret_cast<const float2*>(p.res + off));
+                  v0 = v0 * p.alpha + p.beta * rv.x; v1 = v1 * p.alpha + p.beta * rv.y;
+                }
+              } else if (p.alpha != 1.f) {
+                v0 *= p.alpha; v1 *= p.alpha;
               }
-              const int kchunk = (((rem * CG + (int)rank) * p.mt + g) << 2) + q;
-              float2* wsp = reinterpret_cast<float2*>(p.stats_ws) + ((int64_t)kchunk * p.B + b) * p.Cout + nb + lane;
-              *wsp = make_float2(ssum, ssq);
-            }
-          } else {
-            named_bar_sync(1, 128);
-            if (store_thread) {
-              tma_store_4d(&p.out_map[ph], sbuf, nb, ox0 + g * TILE_W, oy0, b);
-              tma_store_commit();
+              if (p.round_tf32) { v0 = vt_round_tf32(v0); v1 = vt_round_tf32(v1); }
+              if (p.rgb_w) {
+                // 1x1 modulated conv to 3 channels on the values just produced (model/stylegan/model.py:384-385)
+                const float* w0 = p.rgb_w + ((int64_t)(p.wB > 1 ? b : 0) * 3) * p.Cout + ch;
+#pragma unroll
+                for (int cc = 0; cc < 3; ++cc) {
+                  const float2 wv = __ldg(reinterpret_cast<const float2*>(w0 + cc * p.Cout));
+                  rgb[h][cc] = fmaf(v1, wv.y, fmaf(v0, wv.x, rgb[h][cc]));
+                }
+              }
+              if (in_img[h] && p.out) *reinterpret_cast<float2*>(p.out + off) = make_float2(v0, v1);
+              v[h][k][0] = in_img[h] ? v0 : 0.f; v[h][k][1] = in_img[h] ? v1 : 0.f;
             }
           }
+          if (p.stats_ws) {
+            // AdaptiveInstanceNorm statistics of the tensor this launch writes (model/dualstylegan.py:10-21): per channel, the
+            // warp's 16 pixels summed in a fixed butterfly order (no atomics), pixels outside the image masked
+            const int kchunk = ((rem * p.mt + g) * STATS_WARPS) + c * 4 + tw_;
+            float2* wsp = reinterpret_cast<float2*>(p.stats_ws) + ((int64_t)kchunk * p.B + b) * p.Cout + nb + 2 * qd;
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                float ssum = v[0][k][e] + v[1][k][e];
+                float ssq = fmaf(v[0][k][e], v[0][k][e], v[1][k][e] * v[1][k][e]);
+#pragma unroll
+                for (int o = 4; o < 32; o <<= 1) {
+                  ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
+                  ssq += __shfl_xor_sync(0xffffffffu, ssq, o);
+                }
+                if (lane < 4) wsp[8 * k + e] = make_float2(ssum, ssq);
+              }
           }
-          if (p.dbg) tw[3] += clock64() - t_st0;
         }
-        if (p.rgb_w && in_img) {
-          // + bias + Upsample(skip): upfirdn2d(up=2, pad=(2,1), 4x4 kernel) touches exactly 2x2 skip pixels per output
-          // pixel (taps with (y-2+ky) even).  Branch-free: clamped addresses + validity masks so the 12 loads issue together.
-          float o[3] = {rgb0 + __ldg(p.rgb_bias), rgb1 + __ldg(p.rgb_bias + 1), rgb2 + __ldg(p.rgb_bias + 2)};
-          const int64_t HW = (int64_t)p.Ho * p.Wo;
-          if (p.rgb_skip) {
-            const int hs = p.Ho >> 1, ws = p.Wo >> 1;
-            const int ky0 = (oy - 2) & 1, kx0 = (ox - 2) & 1;
-            const int iy0 = (oy - 2 + ky0) >> 1, ix0 = (ox - 2 + kx0) >> 1;        // second tap is +1
-            const float my0 = iy0 >= 0 ? 1.f : 0.f, my1 = (iy0 + 1) < hs ? 1.f : 0.f;
-            const float mx0 = ix0 >= 0 ? 1.f : 0.f, mx1 = (ix0 + 1) < ws ? 1.f : 0.f;
-            const int cy0 = iy0 < 0 ? 0 : iy0, cy1 = (iy0 + 1) < hs ? iy0 + 1 : hs - 1;
-            const int cx0 = ix0 < 0 ? 0 : ix0, cx1 = (ix0 + 1) < ws ? ix0 + 1 : ws - 1;
-            // flipped-kernel weights of the 4 taps (ky in {ky0, ky0+2}, kx in {kx0, kx0+2})
-            const float* kk = p.rgb_skip_kernel;
-            const float w00 = __ldg(kk + (3 - ky0) * 4 + (3 - kx0)) * my0 * mx0;
-            const float w01 = __ldg(kk + (3 - ky0) * 4 + (1 - kx0)) * my0 * mx1;
-            const float w10 = __ldg(kk + (1 - ky0) * 4 + (3 - kx0)) * my1 * mx0;
-            const float w11 = __ldg(kk + (1 - ky0) * 4 + (1 - kx0)) * my1 * mx1;
-            float s00[3], s01[3], s10[3], s11[3];
+        if (p.rgb_w) {
 #pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const float* sp = p.rgb_skip + ((int64_t)b * 3 + c) * (int64_t)hs * ws;
-              s00[c] = __ldg(sp + (int64_t)cy0 * ws + cx0); s01[c] = __ldg(sp + (int64_t)cy0 * ws + cx1);
-              s10[c] = __ldg(sp + (int64_t)cy1 * ws + cx0); s11[c] = __ldg(sp + (int64_t)cy1 * ws + cx1);
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int cc = 0; cc < 3; ++cc) {
+              rgb[h][cc] += __shfl_xor_sync(0xffffffffu, rgb[h][cc], 1);
+              rgb[h][cc] += __shfl_xor_sync(0xffffffffu, rgb[h][cc], 2);
             }
 #pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              // same accumulation order as the reference loop (ky outer, kx inner)
-              float u = s00[c] * w00;
-              u = fmaf(s01[c], w01, u);
-              u = fmaf(s10[c], w10, u);
-              u = fmaf(s11[c], w11, u);
-              o[c] += u;
+          for (int h = 0; h < 2; ++h) {
+            if (qd != 0 || !in_img[h]) continue;
+            const int py = oy[h], px = ox[h];
+            // + bias + Upsample(skip): upfirdn2d(up=2, pad=(2,1), 4x4 kernel) touches exactly 2x2 skip pixels per output
+            // pixel (taps with (y-2+ky) even).  Branch-free: clamped addresses + validity masks so the 12 loads issue together.
+            float o[3] = {rgb[h][0] + __ldg(p.rgb_bias), rgb[h][1] + __ldg(p.rgb_bias + 1), rgb[h][2] + __ldg(p.rgb_bias + 2)};
+            const int64_t HW = (int64_t)p.Ho * p.Wo;
+            if (p.rgb_skip) {
+              const int hs = p.Ho >> 1, ws = p.Wo >> 1;
+              const int ky0 = (py - 2) & 1, kx0 = (px - 2) & 1;
+              const int iy0 = (py - 2 + ky0) >> 1, ix0 = (px - 2 + kx0) >> 1;        // second tap is +1
+              const float my0 = iy0 >= 0 ? 1.f : 0.f, my1 = (iy0 + 1) < hs ? 1.f : 0.f;
+              const float mx0 = ix0 >= 0 ? 1.f : 0.f, mx1 = (ix0 + 1) < ws ? 1.f : 0.f;
+              const int cy0 = iy0 < 0 ? 0 : iy0, cy1 = (iy0 + 1) < hs ? iy0 + 1 : hs - 1;
+              const int cx0 = ix0 < 0 ? 0 : ix0, cx1 = (ix0 + 1) < ws ? ix0 + 1 : ws - 1;
+              // flipped-kernel weights of the 4 taps (ky in {ky0, ky0+2}, kx in {kx0, kx0+2})
+              const float* kk = p.rgb_skip_kernel;
+              const float w00 = __ldg(kk + (3 - ky0) * 4 + (3 - kx0)) * my0 * mx0;
+              const float w01 = __ldg(kk + (3 - ky0) * 4 + (1 - kx0)) * my0 * mx1;
+              const float w10 = __ldg(kk + (1 - ky0) * 4 + (3 - kx0)) * my1 * mx0;
+              const float w11 = __ldg(kk + (1 - ky0) * 4 + (1 - kx0)) * my1 * mx1;
+#pragma unroll
+              for (int cc = 0; cc < 3; ++cc) {
+                const float* sp = p.rgb_skip + ((int64_t)b * 3 + cc) * (int64_t)hs * ws;
+                // same accumulation order as the reference loop (ky outer, kx inner)
+                float u = __ldg(sp + (int64_t)cy0 * ws + cx0) * w00;
+                u = fmaf(__ldg(sp + (int64_t)cy0 * ws + cx1), w01, u);
+                u = fmaf(__ldg(sp + (int64_t)cy1 * ws + cx0), w10, u);
+                u = fmaf(__ldg(sp + (int64_t)cy1 * ws + cx1), w11, u);
+                o[cc] += u;
+              }
             }
+#pragma unroll
+            for (int cc = 0; cc < 3; ++cc) p.rgb_out[((int64_t)b * 3 + cc) * HW + (int64_t)py * p.Wo + px] = o[cc];
           }
-#pragma unroll
-          for (int c = 0; c < 3; ++c) p.rgb_out[((int64_t)b * 3 + c) * HW + (int64_t)oy * p.Wo + ox] = o[c];
         }
       }
-      if (++as == p.acc_stages) { as = 0; t_par ^= 1; }
     }
-    if (p.warp_store ? (lane == 0) : store_thread) tma_store_wait_all<0>();
-  }
-
-  if (p.dbg && lane == 0 && (warp == 0 || warp == 1 || warp == 4)) {
-    const int role = warp == 4 ? 2 : warp;   // 0 producer, 1 mma, 2 epilogue
-    unsigned long long* o = p.dbg + (size_t)blockIdx.x * 16 + role * 5;
-    o[0] = (unsigned long long)(clock64() - t_begin);
-    o[1] = (unsigned long long)tw[0]; o[2] = (unsigned long long)tw[1]; o[3] = (unsigned long long)tw[2]; o[4] = (unsigned long long)tw[3];
-  }
-  if (p.dbg && lane == 0 && warp == 2 && p.bf16x3) p.dbg[(size_t)blockIdx.x * 16 + 15] = (unsigned long long)tw[0];   // transform: wait for TMA
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if (CG == 2) tmem_dealloc_2sm(tmem_base, (uint32_t)p.tmem_cols);
-    else tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
   }
 }
 
@@ -717,23 +572,17 @@ inline int make_map4(CUtensorMap* m, const void* base, const uint64_t dims[4], c
 
 int g_tc_mode = 1;  // 0: one TMA box per tap; 1: one halo box per K chunk + row-shifted descriptors
 int g_tc_mt = 0;    // 0: automatic M-tiles per work item; 1/2/4: forced
-unsigned long long* g_tc_dbg = nullptr;   // device buffer [148][16] set through vt_set_debug_buffer (tuning only)
-int g_tc_cg2 = 1;     // 1: use CTA pairs (cta_group::2, M = 256) for N-tile-256 stride-1 halo convolutions
 int g_tc_transpose = 1;   // 1: hand the problem over transposed when that wastes fewer tiles; 0: never; 2: always (tests)
-int g_tc_pair_y = -1;     // -1: automatic pair orientation; 0/1: forced (tests)
-int g_tc_direct_store = 0;  // epilogue output path: 0 = smem staging + TMA store, 1 = direct 128-byte row stores, 2 = direct for N <= 128
 int g_tc_tgroup = 0;  // 0: automatic taps per weight box (<= 36 KB); 1: one tap per box; n>1: KB budget
-int g_tc_s2_halo = 0;  // 1: stride-2 layers may use halo staging (4 parity-view boxes per K chunk, 78 KB for a 3x3) and with it CTA pairs
+int g_tc_s2_halo = 0;  // 1: stride-2 layers may use halo staging (4 parity-view boxes per K chunk, 78 KB for a 3x3)
 int g_tc_stage_policy = 1;  // big halo boxes (dilated 3x3): 0 = shrink the weight ring first (3 + 3 stages at dilation 4), 1 = keep >= 5 weight stages and drop to 2 halo stages
 int g_tc_halo_pct = 60;    // halo staging must stage at most this percentage of the per-tap bytes (stride 1)
 int g_tc_m_major = 1;      // work items ordered pixel-tile-major (the N tiles of a pixel tile run side by side: the activations' second read hits L2)
-int g_tc_warp_store = 1;   // epilogue: per-warp staging + TMA stores (8 x 4 pixel boxes) instead of one CTA-wide store per chunk
-int g_tc_strict = 1;  // 1: cluster-scope release arrive in the transform warps (no measurable cost here: 74.43 vs 74.41 frames/s); 0: plain remote arrive
 
 int check_supported(const vt_conv_desc* d, bool set_err) {
 #define VT_SUP(cond, ...) do { if (!(cond)) { if (set_err) vt_set_error(__VA_ARGS__); return 0; } } while (0)
   VT_SUP(d->Cout % 32 == 0, "conv_tc: Cout must be a multiple of 32 (got %d)", d->Cout);
-  VT_SUP(d->out != nullptr, "conv_tc: out must not be NULL (the image-only ToRGB form exists in the row-strip kernel only)");
+  VT_SUP(d->out != nullptr || d->rgb_w != nullptr, "conv_tc: out may be NULL only with the fused ToRGB tail (image-only launch)");
   for (int s = 0; s < d->n_src; ++s) {
     VT_SUP(d->src_c[s] % KCH == 0, "conv_tc: src_c[%d]=%d must be a multiple of 32", s, d->src_c[s]);
     VT_SUP(d->src_cstride[s] % 4 == 0, "conv_tc: channel stride must be a multiple of 4");
@@ -753,21 +602,17 @@ int check_supported(const vt_conv_desc* d, bool set_err) {
   VT_SUP(!d->res || (((uintptr_t)d->res & 15) == 0), "conv_tc: res not 16-byte aligned");
   VT_SUP(!d->bias || (((uintptr_t)d->bias & 15) == 0), "conv_tc: bias not 16-byte aligned");
   VT_SUP(!d->slope_vec || (((uintptr_t)d->slope_vec & 15) == 0), "conv_tc: slope_vec not 16-byte aligned");
-  VT_SUP(!d->rgb_w || (d->n_phase == 1 && d->Cout <= 256 && (((uintptr_t)d->rgb_w & 15) == 0) &&
+  // fused ToRGB: every channel of a pixel must be in one N tile (the 3-channel dot product is finished in the epilogue)
+  VT_SUP(!d->rgb_w || (d->n_phase == 1 && d->Cout <= MAX_BLOCK_N && (d->Cout & (d->Cout - 1)) == 0 && (((uintptr_t)d->rgb_w & 15) == 0) &&
                        d->out_sx == d->Cout && d->out_sy == (int64_t)d->Wo * d->Cout && (!d->rgb_skip || (d->Ho % 2 == 0 && d->Wo % 2 == 0))),
-         "conv_tc: fused ToRGB needs Cout <= 256, one phase, a dense output and even Ho/Wo for the skip");
+         "conv_tc: fused ToRGB needs Cout a power of two <= 128, one phase, a dense output and even Ho/Wo for the skip");
   return 1;
 #undef VT_SUP
 }
 
 }  // namespace
 
-int vt_rs_set_option(const char* key, int value, int* old);   // conv_rs.cu
-int vt_rsu_set_option(const char* key, int value, int* old);  // conv_rsu.cu
-
 extern "C" int vt_set_option(const char* key, int value) {
-  { int old = 0; if (vt_rs_set_option(key, value, &old)) return old; }
-  { int old = 0; if (vt_rsu_set_option(key, value, &old)) return old; }
   if (key && strcmp(key, "tc_mode") == 0) { int old = g_tc_mode; g_tc_mode = value; return old; }
   if (key && strcmp(key, "tc_mt") == 0) { int old = g_tc_mt; g_tc_mt = value; return old; }
   if (key && strcmp(key, "tc_tgroup") == 0) { int old = g_tc_tgroup; g_tc_tgroup = value; return old; }
@@ -775,21 +620,13 @@ extern "C" int vt_set_option(const char* key, int value) {
   if (key && strcmp(key, "tc_stage_policy") == 0) { int old = g_tc_stage_policy; g_tc_stage_policy = value; return old; }
   if (key && strcmp(key, "tc_halo_pct") == 0) { int old = g_tc_halo_pct; g_tc_halo_pct = value; return old; }
   if (key && strcmp(key, "tc_m_major") == 0) { int old = g_tc_m_major; g_tc_m_major = value; return old; }
-  if (key && strcmp(key, "tc_warp_store") == 0) { int old = g_tc_warp_store; g_tc_warp_store = value; return old; }
-  if (key && strcmp(key, "tc_strict") == 0) { int old = g_tc_strict; g_tc_strict = value; return old; }
-  if (key && strcmp(key, "tc_direct_store") == 0) { int old = g_tc_direct_store; g_tc_direct_store = value; return old; }
-  if (key && strcmp(key, "tc_cg2") == 0) { int old = g_tc_cg2; g_tc_cg2 = value; return old; }
   if (key && strcmp(key, "tc_transpose") == 0) { int old = g_tc_transpose; g_tc_transpose = value; return old; }
-  if (key && strcmp(key, "tc_pair_y") == 0) { int old = g_tc_pair_y; g_tc_pair_y = value; return old; }
   if (key && strcmp(key, "instnorm_chunks") == 0) { int old = g_instnorm_chunks; g_instnorm_chunks = value; return old; }
   if (key && strcmp(key, "fir4") == 0) { int old = g_fir4; g_fir4 = value; return old; }
   if (key && strcmp(key, "smalln_is") == 0) { int old = g_smalln_is; g_smalln_is = value; return old; }
   if (key && strcmp(key, "upfirdn_tiled") == 0) { int old = g_upfirdn_tiled; g_upfirdn_tiled = value; return old; }
   return -1;
 }
-
-unsigned long long* g_tc_dbg_export = nullptr;   // the same buffer, visible to conv_rs.cu
-extern "C" int vt_set_debug_buffer(void* p) { g_tc_dbg = (unsigned long long*)p; g_tc_dbg_export = g_tc_dbg; return 0; }
 
 extern "C" int vt_conv2d_tc_supported(const vt_conv_desc* d) {
   if (!d || d->struct_size != (int)sizeof(vt_conv_desc)) return 0;
@@ -829,16 +666,12 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
       a.phase_pix[ph] = a.phase_off[ph] / d->out_cpitch;
     }
   }
-  a.dbg = g_tc_dbg;
   a.out = d->out;
-  a.warp_store = g_tc_warp_store ? 1 : 0;
-  a.direct_store = (g_tc_direct_store == 1) || (g_tc_direct_store == 2 && d->n_phase * d->Cout <= 128);
   a.slope_vec = d->slope_vec;
   a.rgb_w = d->rgb_w; a.rgb_bias = d->rgb_bias; a.rgb_skip = d->rgb_skip; a.rgb_skip_kernel = d->rgb_skip_kernel; a.rgb_out = d->rgb_out;
   a.act = d->act; a.round_tf32 = d->round_tf32; a.slope = d->slope; a.gain = d->gain; a.alpha = d->alpha; a.beta = d->beta;
   a.B = d->B;
   a.bf16x3 = d->weight_bf16x3 != nullptr;
-  a.strict_release = g_tc_strict;
   a.fmt = (a.bf16x3 && d->split_fmt == 1) ? 1 : 0;
   a.acc_scale = (a.bf16x3 && d->acc_scale > 0.f) ? d->acc_scale : 1.f;
   a.nstack = (a.bf16x3 && d->bf16x3_nstack) ? 1 : 0;
@@ -870,27 +703,25 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
     dymin = vy < dymin ? vy : dymin; dymax = vy > dymax ? vy : dymax;
   }
 
-  // ---- N tile and accumulator plan (TMEM: 512 columns)
-  // GEMM N = n_phase * Cout (phase-major rows of the weight tensor); N tile = largest multiple of 32 <= 256 dividing it
+  // ---- N tile and accumulator plan (registers: mt * N <= 256 accumulator columns per consumer thread)
+  // GEMM N = n_phase * Cout (phase-major rows of the weight tensor); N tile = largest power of two <= 128 dividing it
   const int n_eff = d->n_phase * d->Cout;
-  int bn = 256;
-  while (bn > 32 && (n_eff % bn) != 0) bn -= 32;
+  int bn = MAX_BLOCK_N;
+  while (bn > 32 && (n_eff % bn) != 0) bn /= 2;
   VT_CHECK(n_eff % bn == 0, "conv_tc: no N tile for N=%d", n_eff);
-  const int bnm = a.nstack ? 2 * bn : bn;   // MMA N = TMEM columns per accumulator = weight rows per tile
+  const int bnm = a.nstack ? 2 * bn : bn;   // MMA N = accumulator columns = weight rows per tile
   // halo staging: multi-tap layers (one box serves all taps) and small-N 1x1 layers (several M tiles per box and weight tile).
   // tc_mode 3: halo for stride 1 only (A/B tests)
   const bool can_halo = (g_tc_mode != 0) && (d->taps > 1 || (bn <= 64 && d->stride == 1)) && (d->stride == 1 || g_tc_mode != 3);
   // M tiles per work item: share each weight tile across `mt` pixel tiles when N is small (weights dominate L2->smem
-  // traffic there); bounded by TMEM columns and by the halo box fitting a pipeline stage.
+  // traffic there); bounded by the accumulator registers and by the halo box fitting a pipeline stage.
   int mt = 1;
   if (can_halo && g_tc_mt != 1) {
-    int want = (g_tc_mt > 0) ? g_tc_mt : (bn >= 256 ? 1 : (bn >= 128 ? 2 : 4));
-    // keep two accumulator stages (epilogue/mainloop overlap) unless forced: 2 * n_phase * mt * bn <= 512 TMEM columns
-    const int col_budget = (g_tc_mt > 0) ? 512 : ((2 * bnm <= 512) ? 256 : 512);
-    while (want > 1 && (want * bnm > col_budget || gWo <= TILE_W * (want / 2))) want /= 2;
+    int want = (g_tc_mt > 0) ? g_tc_mt : (bn >= 128 ? 1 : (bn >= 64 ? 2 : 4));
+    while (want > 1 && (want * bnm > MAX_ACC_COLS || gWo <= TILE_W * (want / 2))) want /= 2;
     mt = want;
   }
-  const int fixed = 2 * STAGING_BYTES + 1024 /*barriers*/ + 1024 /*alignment slack*/;
+  const int fixed = 1024 /*barriers*/ + 1024 /*alignment slack*/;
   int smem_bytes = 0;
   // taps per weight box: as many consecutive slabs as fit ~36 KB, dividing the step count, never crossing a phase
   int tgroup = 1;
@@ -903,16 +734,7 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
       if (ok) { tgroup = tg; break; }
     }
   }
-  // CTA pairs (cta_group::2, one MMA instruction covers M = 256 pixels): stride-1 halo mode. g_tc_cg2: 1 = every eligible
-  // layer (small-N layers are bound by MMA issue, a pair halves the instructions per pixel), 2 = only N tile 256.
-  const int halo1_bytes = d->stride == 1 ? (TILE_W + (dxmax - dxmin)) * (TILE_H + (dymax - dymin)) * 128 : 0;   // (stride 2: decided by the plan below)
-  int cg = (g_tc_cg2 && can_halo && (bn == 256 || g_tc_cg2 == 1) && (gWo > TILE_W * mt || gHo > TILE_H) &&
-            (int64_t)halo1_bytes * 100 <= (int64_t)d->taps * TILE_M * 128 * g_tc_halo_pct && halo1_bytes <= 96 * 1024) ? 2 : 1;
   a.tgroup = tgroup;
-  for (int t = 0; t < d->taps && t < 32; ++t) {
-    if (t % tgroup == 0) a.grp_first_mask |= 1 << t;
-    if (t % tgroup == tgroup - 1) a.grp_last_mask |= 1 << t;
-  }
   // per parity view (stride 1: view 0 only): offset ranges of the taps that read it
   int vx0[4], vx1[4], vy0[4], vy1[4];
   bool vused[4] = {false, false, false, false};
@@ -943,17 +765,16 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
     const int64_t tap_bytes = (int64_t)d->taps * TILE_M * 128;
     const bool pays = (d->stride == 2 && g_tc_s2_halo) ? (tx_bytes * 10 <= tap_bytes * 6) : ((int64_t)tx_bytes * 100 <= tap_bytes * g_tc_halo_pct);
     a.halo = can_halo && fits && halo_bytes <= 96 * 1024 && (mt > 1 || pays) &&
-             2 * halo_bytes + 2 * (bnm / cg) * 128 * tgroup + fixed <= MAX_SMEM;   // at least a 2+2 stage pipeline must fit
+             2 * halo_bytes + 2 * bnm * 128 * tgroup + fixed <= MAX_SMEM;   // at least a 2+2 stage pipeline must fit
     if (!a.halo && mt > 1) continue;
-    if (!a.halo) cg = 1;
     a.halo_x0 = a.hv_x0[0]; a.halo_y0 = a.hv_y0[0]; a.halo_w = hv_w[a.hv_view[0]];
     a.a_tx_bytes = a.halo ? tx_bytes : TILE_M * 128;
     a.a_rows = a.halo ? (a.hv_off[a.n_hv - 1] + a.hv_bytes[a.n_hv - 1]) / 128 : TILE_M;
-    // shared memory plan: A ring (halo boxes or per-tap tiles) + B ring (weight tiles) + 2 output staging buffers
+    // shared memory plan: A ring (halo boxes or per-tap tiles) + B ring (weight tiles)
     a.a_stage_bytes = a.halo ? halo_bytes : TILE_M * 128;
-    a.b_stage_bytes = (bnm / cg) * 128 * tgroup;
+    a.b_stage_bytes = bnm * 128 * tgroup;
     a.a_stages = a.halo ? 3 : 4;
-    a.b_stages = tgroup > 1 ? 4 : (cg == 2 ? 8 : 6);
+    a.b_stages = tgroup > 1 ? 4 : 6;
     // a K chunk's MMAs (taps x 6 instructions) cover one halo stage; a weight stage covers one tap only: with big halo boxes a
     // deeper weight ring hides more TMA latency than a third halo stage (policy 1)
     const int b_floor = (g_tc_stage_policy == 1 && a.halo && a.a_stage_bytes >= 40 * 1024 && tgroup == 1) ? 5 : 3;
@@ -968,7 +789,7 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
     smem_bytes = a.a_stages * a.a_stage_bytes + a.b_stages * a.b_stage_bytes + fixed;
     if (smem_bytes <= MAX_SMEM || mt == 1) break;
   }
-  a.b_tx_bytes = (bnm / cg) * 128 * tgroup;
+  a.b_tx_bytes = bnm * 128 * tgroup;
   VT_CHECK(smem_bytes <= MAX_SMEM && a.a_stages >= 2 && a.b_stages >= 2 && a.a_stages <= 8 && a.b_stages <= 8,
            "conv_tc: shared memory plan does not fit (%d B, mt=%d, bn=%d)", smem_bytes, mt, bn);
   for (int t = 0; t < d->taps; ++t) {
@@ -979,36 +800,26 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
     a.step_sbo[t] = (uint16_t)(hv_w[v] * 128);
   }
   a.mt = mt;
-  a.acc_stages = (2 * mt * bnm <= 512) ? 2 : 1;
-  int tc = 32;
-  while (tc < a.acc_stages * mt * bnm) tc *= 2;
-  a.tmem_cols = tc;
   a.block_n = bn;
   a.mma_n = bnm;
   a.n_tiles = n_eff / bn;
-  // pair orientation: side by side (x) or stacked (y), whichever wastes fewer tiles; ties -> x
-  if (cg == 2) {
-    const int64_t px = vt_cdiv(gWo, TILE_W * mt * 2) * vt_cdiv(gHo, TILE_H), py = vt_cdiv(gWo, TILE_W * mt) * vt_cdiv(gHo, TILE_H * 2);
-    a.pair_y = (g_tc_pair_y >= 0) ? g_tc_pair_y : (py < px ? 1 : 0);
-  }
-  a.tiles_x = (int)vt_cdiv(gWo, TILE_W * mt * ((cg == 2 && !a.pair_y) ? 2 : 1));
-  a.tiles_y = (int)vt_cdiv(gHo, TILE_H * ((cg == 2 && a.pair_y) ? 2 : 1));
+  VT_CHECK(!d->rgb_w || a.n_tiles == 1, "conv_tc: fused ToRGB needs one N tile (Cout = %d)", d->Cout);
+  a.tiles_x = (int)vt_cdiv(gWo, TILE_W * mt);
+  a.tiles_y = (int)vt_cdiv(gHo, TILE_H);
   const int64_t total = (int64_t)a.n_tiles * a.B * a.tiles_x * a.tiles_y;
   VT_CHECK(total < (1LL << 31), "conv_tc: too many tiles");
   a.total_tiles = (int)total;
   a.m_major = g_tc_m_major ? 1 : 0;
   {
-    // fused instance-norm statistics of the output: one chunk per (pixel tile of an image, epilogue warp)
-    const int64_t chunks = (int64_t)a.tiles_x * a.tiles_y * cg * mt * 4;
+    // fused instance-norm statistics of the output: one chunk per (pixel tile of an image, consumer warp)
+    const int64_t chunks = (int64_t)a.tiles_x * a.tiles_y * mt * STATS_WARPS;
     if (chunks_out) {
-      VT_CHECK(a.warp_store && !a.direct_store && d->n_phase == 1 && !d->rgb_w && chunks < (1 << 24),
-               "conv_tc: output statistics need the per-warp store epilogue, one phase and no fused ToRGB");
+      VT_CHECK(d->n_phase == 1 && !d->rgb_w && chunks < (1 << 24), "conv_tc: output statistics need one phase and no fused ToRGB");
       *chunks_out = (int)chunks;
       return 0;
     }
     if (d->stats_ws) {
-      VT_CHECK(a.warp_store && !a.direct_store && d->n_phase == 1 && !d->rgb_w,
-               "conv_tc: output statistics need the per-warp store epilogue, one phase and no fused ToRGB");
+      VT_CHECK(d->n_phase == 1 && !d->rgb_w, "conv_tc: output statistics need one phase and no fused ToRGB");
       VT_CHECK(d->stats_ws_floats >= chunks * d->B * d->Cout * 2, "conv_tc: stats_ws too small (%lld floats, need %lld)",
                (long long)d->stats_ws_floats, (long long)(chunks * d->B * d->Cout * 2));
       VT_CHECK(((uintptr_t)d->stats_ws & 7) == 0, "conv_tc: stats_ws not 8-byte aligned");
@@ -1052,47 +863,29 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
       const uint64_t rows = (uint64_t)n_eff * (a.nstack ? 2 : 1);   // N-stacked: 32 [w_hi|w_hi] rows then 32 [w_lo|w_lo] rows per tap
       const uint64_t dims2[4] = {2 * wc, rows, (uint64_t)d->w_taps, (uint64_t)d->wB};
       const uint64_t str2[3] = {wc * 4, rows * wc * 4, (uint64_t)d->w_taps * rows * wc * 4};
-      const uint32_t box[4] = {2 * KCH, (uint32_t)(bnm / cg), (uint32_t)a.tgroup, 1};
+      const uint32_t box[4] = {2 * KCH, (uint32_t)bnm, (uint32_t)a.tgroup, 1};
       if (make_map4(&a.w_map, d->weight_bf16x3, dims2, str2, box, "weight(bf16x3)", true)) return 1;
     } else {
-      const uint32_t box[4] = {KCH, (uint32_t)(bn / cg), (uint32_t)a.tgroup, 1};
+      const uint32_t box[4] = {KCH, (uint32_t)bn, (uint32_t)a.tgroup, 1};
       if (make_map4(&a.w_map, d->weight, dims, str, box, "weight")) return 1;
     }
   }
-  for (int ph = 0; ph < d->n_phase; ++ph) {
-    const uint64_t dims[4] = {(uint64_t)d->Cout, (uint64_t)gWo, (uint64_t)gHo, (uint64_t)d->B};
-    const uint64_t str[3] = {(uint64_t)g_out_sx * 4, (uint64_t)g_out_sy * 4, (uint64_t)d->out_sb * 4};
-    const uint32_t box[4] = {32, TILE_W, (uint32_t)(a.warp_store ? TILE_H / 4 : TILE_H), 1};
-    if (make_map4(&a.out_map[ph], d->out + d->phase_off[ph], dims, str, box, "output")) return 1;
-  }
-  for (int ph = d->n_phase; ph < 4; ++ph) a.out_map[ph] = a.out_map[0];
-
   static std::once_flag attr_once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(attr_once, [] {
-    attr_err = cudaFuncSetAttribute(conv_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
-    if (attr_err == cudaSuccess)
-      attr_err = cudaFuncSetAttribute(conv_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
+    attr_err = cudaFuncSetAttribute(conv_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
+    if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
+    if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
   });
   VT_CHECK(attr_err == cudaSuccess, "conv_tc: cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err));
-  if (cg == 1) {
-    int grid = vt_num_sms();
-    if (grid > a.total_tiles) grid = a.total_tiles;
-    conv_tc_kernel<1><<<grid, TC_THREADS, smem_bytes, (cudaStream_t)stream>>>(a);
-  } else {
-    int pairs = vt_num_sms() / 2;
-    if (pairs > a.total_tiles) pairs = a.total_tiles;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(2 * pairs));
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = (size_t)smem_bytes;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    VT_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<2>, a));
+  int grid = vt_num_sms();
+  if (grid > a.total_tiles) grid = a.total_tiles;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (bnm) {
+    case 32: conv_tc_kernel<32><<<grid, TC_THREADS, smem_bytes, st>>>(a); break;
+    case 64: conv_tc_kernel<64><<<grid, TC_THREADS, smem_bytes, st>>>(a); break;
+    case 128: conv_tc_kernel<128><<<grid, TC_THREADS, smem_bytes, st>>>(a); break;
+    default: return vt_set_error("conv_tc: no kernel for MMA N = %d", bnm);
   }
   VT_LAUNCH_CHECK();
   return 0;
@@ -1100,180 +893,30 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
 
 extern "C" int vt_conv2d_tc_tf32(const vt_conv_desc* d, void* stream) { return conv_tc_run(d, stream, nullptr); }
 
+// Row-strip entry points: the full-resolution 3x3 / stride 1 layers with Cin, Cout in {32, 64}.  On sm_90a they run the wgmma kernel
+// above (the Blackwell build accumulated rows across input rows in tensor memory, which Hopper does not have).
+static bool rs_shape(const vt_conv_desc* d) {
+  if (d->n_src != 1 || d->stride != 1 || d->taps != 9 || d->n_phase != 1 || d->res || d->slope_vec || !d->weight_bf16x3) return false;
+  if (d->src_scale[0] || d->src_affine[0] || d->alpha != 1.f) return false;
+  if ((d->Cout != 32 && d->Cout != 64) || (d->src_c[0] != 32 && d->src_c[0] != 64)) return false;
+  return d->act == VT_ACT_NONE || d->act == VT_ACT_LRELU;
+}
+
+extern "C" int vt_conv2d_rs_supported(const vt_conv_desc* d) {
+  if (!d || d->struct_size != (int)sizeof(vt_conv_desc)) return 0;
+  return rs_shape(d) && check_supported(d, false);
+}
+
+extern "C" int vt_conv2d_rs(const vt_conv_desc* d, float acc_scale, void* stream) {
+  VT_CHECK(d && d->struct_size == (int)sizeof(vt_conv_desc) && rs_shape(d), "conv2d_rs: not a row-strip layer (3x3, stride 1, Cin/Cout in {32, 64})");
+  vt_conv_desc c = *d;
+  if (acc_scale > 0.f) c.acc_scale = acc_scale;
+  return conv_tc_run(&c, stream, nullptr);
+}
+
 extern "C" int vt_conv2d_tc_stats_chunks(const vt_conv_desc* d) {
   int chunks = 0;
   if (conv_tc_run(d, nullptr, &chunks)) return -1;
   return chunks;
 }
 
-// ---- tcgen05 issue-rate microbenchmark (tuning aid, tests/ and tools/ only) -----------------------------------------
-// One CTA per SM issues `reps` x 4 MMAs (M=128, N, K=8) on zero-filled smem operands.
-// variant bit 0: alternate between two accumulators; bit 1: issue from a converged warp (elect.sync) instead of a
-// lane-0 branch; bit 2: commit + wait after every group of 4 MMAs (round-trip latency); bit 3: rotate the operands over
-// 3 different smem buffers (defeats any operand reuse); bit 4: halo-style A descriptor (row-shifted start, SBO 1280);
-// bit 5: a second warp streams global->smem bulk copies (48 KB per round) concurrently (producer traffic).
-__global__ void __launch_bounds__(128, 1)
-tc_issue_bench_kernel(float* out, const float* scratch, int N, int reps, int variant) {
-  extern __shared__ uint8_t smem_raw[];
-  constexpr uint32_t OPB = 24576 + 32768;                       // one operand set: A (halo-sized) + B
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar = base + 3 * OPB, bar2 = bar + 8, slot = bar + 16, dump = base + 3 * OPB + 1024;
-  uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  for (int i = threadIdx.x; i < (int)(3 * OPB / 4); i += blockDim.x) reinterpret_cast<float*>(gen)[i] = 0.f;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) { mbar_init(bar, 1); mbar_init(bar2, 1); fence_barrier_init(); }
-  fence_proxy_async_smem();
-  if (warp == 1) { tmem_alloc(slot, 512); tc_fence_before(); }
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(gen + (slot - base));
-  volatile int* stop = reinterpret_cast<volatile int*>(gen + (slot + 8 - base));
-  if (threadIdx.x == 0) *stop = 0;
-  __syncthreads();
-  long long t0 = 0, t1 = 0;
-  if (warp == 0) {
-    const uint32_t idesc = make_idesc_tf32(128, N);
-    uint32_t phase = 0;
-    const bool converged = variant & 2;
-    if (converged || lane == 0) {
-      t0 = clock64();
-      for (int r = 0; r < reps; ++r) {
-        const uint32_t ob = base + ((variant & 8) ? (uint32_t)(r % 3) * OPB : 0u);
-        const uint64_t adesc = (variant & 16) ? make_smem_desc_sw128(ob + (uint32_t)((r % 3) * 10 + (r % 2)) * 128u, 1280, 0)
-                                              : make_smem_desc_sw128(ob, 1024, 0);
-        const uint64_t bdesc = make_smem_desc_sw128(ob + 24576, 1024, 0);
-        const uint32_t d = tmem + ((variant & 1) ? (uint32_t)((r & 1) * N) : 0u);
-        if (converged) {
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_tf32(d, adesc + 2 * k, bdesc + 2 * k, idesc, 1);
-          }
-          __syncwarp();
-        } else {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_tf32(d, adesc + 2 * k, bdesc + 2 * k, idesc, 1);
-        }
-        if (variant & 4) {
-          if (!converged || elect_one()) umma_commit(bar);
-          mbar_wait(bar, phase, 99);
-          phase ^= 1;
-        }
-      }
-      if (!(variant & 4)) {
-        if (!converged || elect_one()) umma_commit(bar);
-        mbar_wait(bar, phase, 98);
-      }
-      t1 = clock64();
-    }
-    if (lane == 0) *stop = 1;
-    if (lane == 0 && blockIdx.x == 0) { out[0] = (float)(t1 - t0) / (float)(reps * 4); }
-  } else if (warp == 2 && (variant & 32)) {
-    // producer-like traffic: 1-D bulk copies global -> smem into a dump buffer, back to back
-    if (lane == 0) {
-      uint32_t ph = 0;
-      const float* src = scratch + (size_t)blockIdx.x * 12288;
-      long long bytes = 0;
-      while (!*stop) {
-        mbar_arrive_expect_tx(bar2, 49152);
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(dump), "l"(src), "r"(49152), "r"(bar2) : "memory");
-        mbar_wait(bar2, ph, 97);
-        ph ^= 1;
-        bytes += 49152;
-      }
-      if (blockIdx.x == 0) out[1] = (float)bytes;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem, 512); }
-}
-
-// ---- TMEM access-rate probe (tuning aid): 4 warps (one per lane quadrant) run `reps` rounds of 4 x tcgen05.ld / tcgen05.st of
-// 32 columns each. mode 0: ld + wait after every load; 1: 4 loads in flight, one wait; 2: st (zeros) + wait::st per store;
-// 3: 4 stores, one wait. out[0] = cycles per 32-column access of one warp with all 4 warps active.
-__device__ __forceinline__ void tmem_ld_32x32_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_zero_32x32(uint32_t taddr) {
-  const uint32_t z = 0u;
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};"
-      ::"r"(taddr), "r"(z)
-      : "memory");
-}
-__global__ void __launch_bounds__(128, 1)
-tmem_probe_kernel(float* out, int reps, int mode) {
-  __shared__ uint32_t slot;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0) { tmem_alloc(smem_u32(&slot), 512); tc_fence_before(); }
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = slot + ((uint32_t)(warp * 32) << 16);
-  for (int c = 0; c < 512; c += 32) tmem_st_zero_32x32(tmem + c);
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-  __syncthreads();
-  uint32_t acc = 0;
-  const long long t0 = clock64();
-  for (int r = 0; r < reps; ++r) {
-    if (mode == 0) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        uint32_t v[32];
-        tmem_ld_32x32_nowait(tmem + (uint32_t)(((r * 4 + k) & 15) * 32), v);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        acc += v[lane];
-      }
-    } else if (mode == 1) {
-      uint32_t v0[32], v1[32], v2[32], v3[32];
-      tmem_ld_32x32_nowait(tmem + (uint32_t)(((r * 4 + 0) & 15) * 32), v0);
-      tmem_ld_32x32_nowait(tmem + (uint32_t)(((r * 4 + 1) & 15) * 32), v1);
-      tmem_ld_32x32_nowait(tmem + (uint32_t)(((r * 4 + 2) & 15) * 32), v2);
-      tmem_ld_32x32_nowait(tmem + (uint32_t)(((r * 4 + 3) & 15) * 32), v3);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      acc += v0[lane] + v1[(lane + 1) & 31] + v2[(lane + 2) & 31] + v3[(lane + 3) & 31];
-    } else if (mode == 2) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        tmem_st_zero_32x32(tmem + (uint32_t)(((r * 4 + k) & 15) * 32));
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      }
-    } else {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) tmem_st_zero_32x32(tmem + (uint32_t)(((r * 4 + k) & 15) * 32));
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    }
-  }
-  const long long t1 = clock64();
-  if (threadIdx.x == 0 && blockIdx.x == 0) out[0] = (float)(t1 - t0) / (float)(reps * 4);
-  if (acc == 0xdeadbeefu) out[1] = 1.f;
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) { tc_fence_after(); tmem_dealloc(slot, 512); }
-}
-
-extern "C" int vt_selftest_tc_gemm(const float* A, const float*, float* D, int, int N, int K, int variant, void* stream) {
-  if (variant & 64) {   // TMEM access-rate probe: N = mode (0..3), K = reps
-    VT_CHECK(D && K >= 1 && N >= 0 && N <= 3, "selftest_tc_gemm: TMEM probe needs D, reps >= 1, mode 0..3");
-    tmem_probe_kernel<<<vt_num_sms(), 128, 0, (cudaStream_t)stream>>>(D, K, N);
-    VT_LAUNCH_CHECK();
-    return 0;
-  }
-  VT_CHECK(D && N >= 16 && N <= 256 && N % 16 == 0 && K >= 1, "selftest_tc_gemm: D (device float[2]) / N / reps invalid");
-  VT_CHECK(!(variant & 32) || A, "selftest_tc_gemm: variant bit 5 needs a scratch buffer A of 148*48 KB");
-  const int smem = 3 * (24576 + 32768) + 1024 + 49152 + 1024;
-  VT_CUDA(cudaFuncSetAttribute(tc_issue_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  tc_issue_bench_kernel<<<vt_num_sms(), 128, smem, (cudaStream_t)stream>>>(D, A, N, K, variant);
-  VT_LAUNCH_CHECK();
-  return 0;
-}

@@ -414,7 +414,7 @@ upfirdn2d_stream_kernel(const __grid_constant__ UsArgs p) {
       for (int s = 0; s < n_st; ++s, ++it) {
         const int slot = (int)(it % (uint32_t)US_STAGES);
         const uint32_t ph = (it / (uint32_t)US_STAGES) & 1u;
-        mbar_wait(empty_bar(slot), ph ^ 1u, 40);
+        mbar_wait(empty_bar(slot), ph ^ 1u);
         float* const sstage = ring + (size_t)slot * stage_floats;
         const int r = s * US_RS + lane;
         const int iy = g.iy_first + r;
@@ -498,7 +498,7 @@ upfirdn2d_stream_kernel(const __grid_constant__ UsArgs p) {
       const bool vec = out16 && ox + 3 < p.out_w;
       for (int s = 0; s < n_st; ++s, ++it) {
         const int slot = (int)(it % (uint32_t)US_STAGES);
-        mbar_wait(full_bar(slot), (it / (uint32_t)US_STAGES) & 1u, 41);
+        mbar_wait(full_bar(slot), (it / (uint32_t)US_STAGES) & 1u);
         const float* srow = ring + (size_t)slot * stage_floats + 4 * tid;
         const int r0 = s * US_RS - 3;
 #define US_BLUR_ROW(SEPV, RRV)                                                                                   \
@@ -554,7 +554,7 @@ upfirdn2d_stream_kernel(const __grid_constant__ UsArgs p) {
       const unsigned r_span = (unsigned)(g.n_rows - 3);
       for (int s = 0; s < n_st; ++s, ++it) {
         const int slot = (int)(it % (uint32_t)US_STAGES);
-        mbar_wait(full_bar(slot), (it / (uint32_t)US_STAGES) & 1u, 42);
+        mbar_wait(full_bar(slot), (it / (uint32_t)US_STAGES) & 1u);
         const float* srow = ring + (size_t)slot * stage_floats + g.colbase + 2 * tid;
         const int r0 = s * US_RS - 3;
 #pragma unroll
@@ -602,7 +602,7 @@ upfirdn2d_stream_kernel(const __grid_constant__ UsArgs p) {
       const bool vec = out16 && X + 7 < p.out_w;
       for (int s = 0; s < n_st; ++s, ++it) {
         const int slot = (int)(it % (uint32_t)US_STAGES);
-        mbar_wait(full_bar(slot), (it / (uint32_t)US_STAGES) & 1u, 43);
+        mbar_wait(full_bar(slot), (it / (uint32_t)US_STAGES) & 1u);
         const float* srow = ring + (size_t)slot * stage_floats + 4 * tid;
 #define US_UP_ROW(Q0V)                                                                \
         switch (off & 3u) {                                                           \

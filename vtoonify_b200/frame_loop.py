@@ -1,4 +1,4 @@
-"""Frame loop (the hot loop of style_transfer.py:99-183) for batches of frames, B200-style.
+"""Frame loop (the hot loop of style_transfer.py:99-183) for batches of frames.
 
 Reference behaviour per batch: stack frames -> BiSeNet parsing of the 2x up-sampled frames -> ``inputs = cat(x, x_p/16)``
 -> ``y = vtoonify(inputs, s_w.repeat(B,1,1), d_s)`` -> ``clamp(-1,1)`` -> per frame ``tensor2cv2(y[k].cpu())``

@@ -1,6 +1,6 @@
 """``conv2d_gradfix.conv2d`` / ``conv_transpose2d`` — same call signatures as model/stylegan/op/conv2d_gradfix.py:22-75.
 In the reference these forward to cuDNN (F.conv2d / F.conv_transpose2d) on any modern torch; here they run the
-library's NHWC convolution kernels (tcgen05 when shapes allow, fp32 FFMA otherwise).  Forward only.
+library's NHWC convolution kernels (wgmma when shapes allow, fp32 FFMA otherwise).  Forward only.
 
 Supported
   * ``conv2d``: kernels of up to 36 taps (any kh x kw), per-axis padding / dilation, stride s (same on both axes),

@@ -1,4 +1,4 @@
-"""Functional layer over the C-ABI: every function launches hand-written sm_100a kernels from
+"""Functional layer over the C-ABI: every function launches hand-written sm_90a kernels from
 libvtoonify_b200.so on torch CUDA tensors (torch is used for memory and streams only).
 
 Internal activation layout is NHWC (``[B, H, W, C]`` contiguous fp32); the reference-facing modules
@@ -16,11 +16,11 @@ from ._lib import ACT_LRELU, ACT_NONE, ACT_RELU_TANH, ConvDesc, SmallNDesc, chec
 SQRT2 = math.sqrt(2.0)
 
 # Convolution arithmetic (set_precision):
-# "bf16x3" (default, the product path): tcgen05 tensor-core convolutions with every fp32 operand split into bf16 hi + lo parts
+# "bf16x3" (default, the product path): wgmma tensor-core convolutions with every fp32 operand split into bf16 hi + lo parts
 #   (pixels in shared memory, weights by vt_split_weights_bf16x3) and three MMA products per K step, fp32 accumulate:
-#   a_hi*w_hi + a_lo*w_hi + a_hi*w_lo.  Meets the 1e-3 per-pixel parity bar (measured 3.4e-4 end to end).
-# "tf32": the same kernel with TF32 operands: ~7 % faster end to end, but 10-bit mantissas put the ~47-layer VToonify-D output
-#   3-4e-3 away from the fp32 reference (measured), above the parity bar.  Opt-in.
+#   a_hi*w_hi + a_lo*w_hi + a_hi*w_lo.  Meets the 1e-3 per-pixel parity bar (tests/test_gpu_vtoonify.py, test_gpu_fullsize.py).
+# "tf32": the same kernel with TF32 operands: fewer MMA products, but 10-bit mantissas put the ~47-layer VToonify-D output
+#   above the parity bar.  Opt-in.
 # "fp32": every convolution on the fp32-exact FFMA kernel (used to cross-check the tensor-core paths).
 DEFAULT_PRECISION = "bf16x3"
 _precision = DEFAULT_PRECISION
@@ -40,23 +40,20 @@ def get_precision() -> str:
 
 # algorithm switches (kept so tests can compare both formulations on the GPU)
 # fold_upconv: True = always fold Blur o conv_transpose into one N = 4*Cout convolution; an int = only when Cin <= that value
-# (the folded form issues 4x the MMA work but has no intermediate tensor: measured faster for Cin <= 128, slower from Cin = 256 up:
-# tools/upconv_bench.py).  fuse_mask_mul: Fusion's f_E * m_E is applied inside the consumers instead of being materialised.
-# rs_conv: route 3x3 / stride 1 / padding 1 layers with Cin, Cout in {32, 64} and at least rs_min_width pixels per row to the
-# row-strip kernel (vertical taps stacked along N, cross-row accumulation in TMEM: conv_rs.cu); rs_fmt: its operand split
-# ("bf16" | "f16": fp16 halves carry 11 + 11 mantissa bits instead of 8 + 8, weights pre-scaled by 2^10).
+# (the folded form issues 4x the MMA work but has no intermediate tensor; tools/upconv_bench.py compares the two; the threshold
+# of 128 has not been re-measured on H100).  fuse_mask_mul: Fusion's f_E * m_E is applied inside the consumers instead of being materialised.
+# rs_conv: 3x3 / stride 1 / padding 1 layers with Cin, Cout in {32, 64} and at least rs_min_width pixels per row go through the
+# row-strip entry point (vt_conv2d_rs), which can also produce the fused ToRGB image alone; rs_fmt: the operand split of the
+# tensor-core mode ("bf16" | "f16": fp16 halves carry 11 + 11 mantissa bits instead of 8 + 8, weights pre-scaled by F16_WEIGHT_SCALE).
 _options = {"fold_upconv": 128, "fuse_torgb": True, "fuse_mask_mul": True, "smalln_via_tc": True, "bf16x3_nstack": False, "fuse_adain": True,
             "rs_conv": True, "rs_min_width": 256, "rs_fmt": _os.environ.get("VT_SPLIT_FMT", "bf16"), "nvtx": bool(_os.environ.get("VT_NVTX")),
-            # rsu_conv: up-convolutions with Cin <= rsu_max_cin and rows of >= rs_min_width pixels on the row-strip up-conv kernel
-            # (horizontal blur folded into the weights, vertical blur on the TMEM accumulators: conv_rsu.cu)
+            # rsu_conv: up-convolutions with Cin <= rsu_max_cin and rows of >= rs_min_width pixels go through conv_up2_rs_nhwc
             "rsu_conv": True, "rsu_max_cin": 128,
             # fuse_stats: AdaIN statistics of a conv output come from the producing kernel's epilogue (per-tile partial sums + finalize)
             # instead of a separate pass over the tensor
             "fuse_stats": True}
 if _os.environ.get("VT_FOLD_UPCONV_MAX_CIN"):
     _options["fold_upconv"] = int(_os.environ["VT_FOLD_UPCONV_MAX_CIN"])
-if _os.environ.get("VT_RSU_MAX_CIN"):
-    _options["rsu_max_cin"] = int(_os.environ["VT_RSU_MAX_CIN"])      # tuning experiments only
 
 
 def use_folded_upconv(cin: int) -> bool:
@@ -64,7 +61,7 @@ def use_folded_upconv(cin: int) -> bool:
     return bool(v) if isinstance(v, bool) else cin <= int(v)
 
 
-_OPTION_ALIASES = {"split_fmt": "rs_fmt"}   # one split format for all three tensor-core kernels
+_OPTION_ALIASES = {"split_fmt": "rs_fmt"}
 
 
 def set_option(name: str, value) -> None:
@@ -490,43 +487,21 @@ def conv2d_nhwc(srcs: Sequence[torch.Tensor], weight: torch.Tensor, taps, stride
                     raise _lib.VtError("conv2d_nhwc: src_affine must be a contiguous [B, C, 2] table")
                 d.src_affine[i] = af.data_ptr()
     lib = _lib.load()
-    if (prec == "bf16x3" and _options["rs_conv"] and W >= _options["rs_min_width"] and len(srcs) == 1 and phase_offs is None
-            and stride == 1 and len(taps) == 9 and res is None and slope_vec is None and src_scale is None and src_affine is None
-            and Cout in (32, 64) and int(d.src_c[0]) in (32, 64) and w_cs == int(d.src_c[0]) and alpha == 1.0
-            and act in (ACT_NONE, ACT_LRELU)):
-        # full-resolution small-channel 3x3 layer: the row-strip kernel (falls through when the descriptor is not eligible)
-        fmt = _options["rs_fmt"]
-        wrs, acc_scale = rs_weights(weight, fmt)
-        d.weight_bf16x3 = wrs.data_ptr()
-        d.bf16x3_nstack = 3 if fmt == "f16" else 2
-        if lib.vt_conv2d_rs_supported(d):
-            if _tc_profile is not None:
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                cin = int(d.src_c[0])
-                flops = 2.0 * B * Ho * Wo * Cout * cin * 9
-                nbytes = 4.0 * (B * H * W * cin + B * Ho * Wo * (Cout if out is not None else 3) + weight.numel())
-                e0.record()
-                check(lib.vt_conv2d_rs(d, acc_scale, _stream()))
-                e1.record()
-                _tc_profile.append((e0, e1, flops, nbytes, f"{cin}->{Cout} k9 s1 {H}x{W} [row-strip{'' if out is not None else ', image only'}]", 3.0 * flops))
-            else:
-                check(lib.vt_conv2d_rs(d, acc_scale, _stream()))
-            if want_stats:
-                return out, instnorm_stats(out, eps=stats_eps)
-            return out if rgb is None else (out, rgb_out)
-        d.weight_bf16x3 = None
-        d.bf16x3_nstack = 0
-    if out is None:
+    if prec == "bf16x3":
+        d.weight_bf16x3 = weight.data_ptr()   # marks the mode for the *_supported checks; the split buffer is attached below
+    # full-resolution small-channel 3x3 layer: the row-strip entry point (the only route that takes an image-only ToRGB launch)
+    rs = (prec == "bf16x3" and _options["rs_conv"] and W >= _options["rs_min_width"] and len(srcs) == 1 and phase_offs is None
+          and stride == 1 and len(taps) == 9 and res is None and slope_vec is None and src_scale is None and src_affine is None
+          and Cout in (32, 64) and int(d.src_c[0]) in (32, 64) and w_cs == int(d.src_c[0]) and alpha == 1.0
+          and act in (ACT_NONE, ACT_LRELU) and bool(lib.vt_conv2d_rs_supported(d)))
+    if out is None and not rs:
         out = torch.empty((B, Ho, Wo, Cout), device=srcs[0].device, dtype=torch.float32)
         d.out = out.data_ptr()
-    if prec == "bf16x3":
-        d.weight_bf16x3 = weight.data_ptr()   # marks the mode for vt_conv2d_tc_supported; the split buffer is attached below
-    use_tc = prec in ("tf32", "bf16x3") and lib.vt_conv2d_tc_supported(d)
+    use_tc = rs or (prec in ("tf32", "bf16x3") and lib.vt_conv2d_tc_supported(d))
     d.weight_bf16x3 = None
     if use_tc and prec == "bf16x3":
-        # Cout == 32: the N-stacked form needs 4 instead of 6 MMA instructions per tap (and keeps all four hi/lo products);
-        # measured on B200 it is no faster end to end (the epilogue's second TMEM load + add becomes the limiter: DESIGN.md
-        # section 4), so it is off by default
+        # Cout == 32: the N-stacked form needs 4 instead of 6 MMA instructions per tap (and keeps all four hi/lo products) but
+        # twice the accumulator columns; off by default
         nstack = bool(_options["bf16x3_nstack"]) and Cout == 32 and phase_offs is None
         if _options["rs_fmt"] == "f16" and not nstack:
             d.weight_bf16x3 = split_weights_f16x3(weight).data_ptr()
@@ -549,14 +524,14 @@ def conv2d_nhwc(srcs: Sequence[torch.Tensor], weight: torch.Tensor, taps, stride
             flops = 2.0 * B * Ho * Wo * Cout * cin * len(taps)   # algorithmic (the folded up-conv issues 4x this)
             nbytes = 4.0 * (B * H * W * cin + B * Ho * Wo * Cout * d.n_phase + weight.numel())
             e0.record()
-            check(lib.vt_conv2d_tc_tf32(d, _stream()))
+            check(lib.vt_conv2d_rs(d, 0.0, _stream()) if rs else lib.vt_conv2d_tc_tf32(d, _stream()))
             e1.record()
             # MMA flops actually issued: 3 bf16 products per algorithmic product in the split-operand mode, and the folded
             # up-convolution evaluates all 4 output phases with full 3x3 support (4x the transposed conv's algorithmic MACs)
             issued = flops * (3.0 if prec == "bf16x3" else 1.0) * (4.0 if d.n_phase == 4 else 1.0)
             _tc_profile.append((e0, e1, flops, nbytes, f"{cin}->{Cout}{'x4up' if d.n_phase > 1 else ''} k{len(taps)} s{stride} {H}x{W}", issued))
         else:
-            check(lib.vt_conv2d_tc_tf32(d, _stream()))
+            check(lib.vt_conv2d_rs(d, 0.0, _stream()) if rs else lib.vt_conv2d_tc_tf32(d, _stream()))
     else:
         check(lib.vt_conv2d_direct_f32(d, _stream()))
     if want_stats:
@@ -588,31 +563,6 @@ def split_weights_bf16x3(weight: torch.Tensor, nstack: bool = False) -> torch.Te
     return out
 
 
-def rs_weights(weight: torch.Tensor, fmt: str = "bf16"):
-    """``weight`` [wB, 9, Cout, Cin] (prep layout, tap = ky*3 + kx, Cin in {32, 64}) -> (buffer, acc_scale) for vt_conv2d_rs:
-    rows ordered [wB][Cin/32][kx][block = 2 - ky][Cout], each a 32-channel chunk split into 16-bit hi | lo halves.
-    Cached on the tensor object like :func:`split_weights_bf16x3`."""
-    ver = weight._version
-    cached = getattr(weight, "_vt_rs", None)
-    if cached is not None and cached[0] == ver and cached[1] == weight.data_ptr() and cached[2] == fmt:
-        return cached[3], cached[4]
-    wB, nine, Cout, Cin = weight.shape
-    if nine != 9 or Cin % 32 != 0 or not weight.is_contiguous():
-        raise _lib.VtError("rs_weights: needs contiguous [wB, 9, Cout, Cin] weights with Cin a multiple of 32")
-    KC = Cin // 32
-    w = weight.view(wB, 3, 3, Cout, KC, 32).flip(1).permute(0, 4, 2, 1, 3, 5).contiguous()   # [wB, KC, kx, 2-ky, Cout, 32]
-    rows = w.numel() // 32
-    out = torch.empty((rows, 32), device=weight.device, dtype=torch.float32)
-    if fmt == "f16":
-        check(_lib.load().vt_split_weights_f16x3(w.data_ptr(), out.data_ptr(), rows, 32, F16_WEIGHT_SCALE, _stream()))
-        acc_scale = 1.0 / F16_WEIGHT_SCALE
-    else:
-        check(_lib.load().vt_split_weights_bf16x3(w.data_ptr(), out.data_ptr(), rows, 32, 0, _stream()))
-        acc_scale = 1.0
-    weight._vt_rs = (ver, weight.data_ptr(), fmt, out, acc_scale)
-    return out, acc_scale
-
-
 def split_weights_f16x3(weight: torch.Tensor) -> torch.Tensor:
     """fp16 counterpart of :func:`split_weights_bf16x3`: chunks hold ``[half(w * 256) | half(w * 256 - hi)]``; cached on the tensor."""
     ver = weight._version
@@ -639,8 +589,8 @@ def scale_fusable(precision: Optional[str] = None) -> bool:
 
 
 def rgb_fusable(Cout: int, precision: Optional[str] = None) -> bool:
-    """The ToRGB tail can ride in the conv epilogue when one N tile holds all channels (tensor-core path only)."""
-    return (precision or _precision) in ("tf32", "bf16x3") and Cout % 32 == 0 and Cout <= 256 and _options["fuse_torgb"]
+    """The ToRGB tail can ride in the conv epilogue when one N tile (at most 128 channels) holds all channels (tensor-core path only)."""
+    return (precision or _precision) in ("tf32", "bf16x3") and Cout % 32 == 0 and Cout <= 128 and (Cout & (Cout - 1)) == 0 and _options["fuse_torgb"]
 
 
 def conv_out_size(n: int, k: int, stride: int, padding: int, dilation: int) -> int:
@@ -700,72 +650,25 @@ def conv_up2_folded_nhwc(x: torch.Tensor, w_folded: torch.Tensor, bias=None, noi
     return out
 
 
-def separable_blur_taps(kernel: torch.Tensor):
-    """4x4 blur buffer ``K = outer(gk, gk)`` -> the flipped 1-D taps ``g[m] = gk[3 - m]`` as 4 host floats, or None when ``K`` is
-    not such an outer product (checked once per tensor object: one device -> host read)."""
-    cached = getattr(kernel, "_vt_g1d", None)
-    if cached is not None and cached[0] == kernel._version:
-        return cached[1]
-    g = None
-    if tuple(kernel.shape) == (4, 4):
-        K = kernel.detach().double().cpu()
-        tot = float(K.sum())
-        if tot > 0:
-            gk = K.sum(0) / math.sqrt(tot)
-            if float((torch.outer(gk, gk) - K).abs().max()) <= 1e-6 * float(K.abs().max()):
-                g = tuple(float(v) for v in gk.flip(0))
-    kernel._vt_g1d = (kernel._version, g)
-    return g
-
-
 def rsu_eligible(cin: int, cout: int, W: int, kernel: torch.Tensor, pad, precision: Optional[str] = None) -> bool:
     return ((precision or _precision) == "bf16x3" and _options["rsu_conv"] and cin % 32 == 0 and 32 <= cin <= _options["rsu_max_cin"]
             and cout % 32 == 0 and 32 <= cout <= 128 and W >= _options["rs_min_width"] and tuple(pad) == (1, 1)
-            and separable_blur_taps(kernel) is not None)
+            and tuple(kernel.shape) == (4, 4))
 
 
 def conv_up2_rs_nhwc(x: torch.Tensor, w9: torch.Tensor, blur_kernel: torch.Tensor, bias=None, noise=None, noise_w=None,
                      act: int = ACT_NONE, slope: float = 0.2, gain: float = 1.0) -> torch.Tensor:
-    """Blur(conv_transpose2d(x, w, stride 2)) on the row-strip up-conv kernel.  ``w9``: modulated weights ``[wB, 9, Cout, Cin]``
-    (un-rounded fp32, slab ky*3+kx); the folded + split form is cached on the tensor object."""
+    """Blur(conv_transpose2d(x, w, stride 2)) for the full-resolution up-convolutions.  ``w9``: modulated weights ``[wB, 9, Cout, Cin]``
+    (un-rounded fp32, slab ky*3+kx).  The blur is folded into the 4 output-phase kernels (cached on the tensor object) and the layer
+    runs as one wgmma convolution with N = 4 * Cout (:func:`conv_up2_folded_nhwc`)."""
     _req_cuda(x, w9, bias, noise, noise_w)
-    B, H, W, Cin = x.shape
-    wB, nine, Cout, wc = w9.shape
-    g = separable_blur_taps(blur_kernel)
-    if g is None or nine != 9 or wc != Cin or not x.is_contiguous() or not w9.is_contiguous():
-        raise _lib.VtError("conv_up2_rs_nhwc: needs a separable 4x4 blur, [wB, 9, Cout, Cin] weights and a contiguous NHWC input")
-    lib = _lib.load()
-    garr = (_lib.c_float * 4)(*g)
-    fmt = _options["rs_fmt"]
     cached = getattr(w9, "_vt_rsu", None)
-    if cached is not None and cached[0] == w9._version and cached[1] == w9.data_ptr() and cached[2] == fmt and cached[3] == g:
-        wsplit, acc_scale = cached[4], cached[5]
+    if cached is not None and cached[0] == w9._version and cached[1] == w9.data_ptr() and cached[2] is blur_kernel:
+        wf = cached[3]
     else:
-        n = wB * (Cout // 32) * (Cin // 32) * 3 * 192 * 32
-        folded = torch.empty((n // 32, 32), device=x.device, dtype=torch.float32)
-        check(lib.vt_fold_upconv_x_weights_f32(w9.data_ptr(), garr, folded.data_ptr(), wB, Cout, Cin, _stream()))
-        wsplit = torch.empty_like(folded)
-        if fmt == "f16":
-            check(lib.vt_split_weights_f16x3(folded.data_ptr(), wsplit.data_ptr(), n // 32, 32, F16_WEIGHT_SCALE, _stream()))
-            acc_scale = 1.0 / F16_WEIGHT_SCALE
-        else:
-            check(lib.vt_split_weights_bf16x3(folded.data_ptr(), wsplit.data_ptr(), n // 32, 32, 0, _stream()))
-            acc_scale = 1.0
-        w9._vt_rsu = (w9._version, w9.data_ptr(), fmt, g, wsplit, acc_scale)
-    out = torch.empty((B, 2 * H, 2 * W, Cout), device=x.device, dtype=torch.float32)
-    args = (x.data_ptr(), wsplit.data_ptr(), out.data_ptr(), B, H, W, Cin, Cout, wB, garr, _ptr(bias), _ptr(noise), _ptr(noise_w), act,
-            slope, gain, 1 if fmt == "f16" else 0, acc_scale, _stream())
-    if _tc_profile is not None:
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        flops = 2.0 * B * H * W * Cout * Cin * 9
-        nbytes = 4.0 * (B * H * W * Cin + B * 4 * H * W * Cout + w9.numel())
-        e0.record()
-        check(lib.vt_conv_up2_rs(*args))
-        e1.record()
-        _tc_profile.append((e0, e1, flops, nbytes, f"{Cin}->{Cout}x2up k9 s1 {H}x{W} [row-strip up]", 3.0 * 2.0 * flops))
-    else:
-        check(lib.vt_conv_up2_rs(*args))
-    return out
+        wf = fold_upconv_weights(w9, blur_kernel)
+        w9._vt_rsu = (w9._version, w9.data_ptr(), blur_kernel, wf)
+    return conv_up2_folded_nhwc(x, wf, bias=bias, noise=noise, noise_w=noise_w, act=act, slope=slope, gain=gain)
 
 
 def fir_nhwc(x: torch.Tensor, kernel: torch.Tensor, pad: Tuple[int, int], bias: Optional[torch.Tensor] = None,

@@ -1,5 +1,5 @@
 """StyleGAN2 modules with the reference's constructor signatures, forward signatures and state_dict keys
-(model/stylegan/model.py), running on the library's sm_100a kernels.
+(model/stylegan/model.py), running on the library's sm_90a kernels.
 
 Differences in *how* (not what):
   * activations travel NHWC (channels_last); modules accept any NCHW tensor and return logical-NCHW
@@ -214,7 +214,6 @@ class ModulatedConv2d(nn.Module):
             if k != 3:
                 raise NotImplementedError("upsampling ModulatedConv2d is 3x3 in StyleGAN2")
             if externalweight is None and Cs == self.in_channel and ops.rsu_eligible(self.in_channel, self.out_channel, W, self.blur.kernel, self.blur.pad):
-                # row-strip up-conv: horizontal blur folded into the weights, vertical blur on the accumulators (2x, not 4x, the MACs)
                 w9 = self.modulated_weights(style, Cs, None, round_tf32=False)
                 return ops.conv_up2_rs_nhwc(x, w9, self.blur.kernel, bias=bias, noise=noise, noise_w=noise_w, act=a, slope=slope, gain=gain)
             if tuple(self.blur.kernel.shape) == (4, 4) and tuple(self.blur.pad) == (1, 1) and ops.use_folded_upconv(self.in_channel):

@@ -1,7 +1,7 @@
 """VToonify (model/vtoonify.py:92-286) — same constructor, ``forward(x, style, d_s=None, return_mask=False,
-return_feat=False)``, ``stylegan()``, ``zplus2wplus()`` and state_dict keys, on the library's sm_100a kernels.
+return_feat=False)``, ``stylegan()``, ``zplus2wplus()`` and state_dict keys, on the library's sm_90a kernels.
 
-The forward keeps every activation NHWC and issues, per layer, one tcgen05 implicit-GEMM convolution with the layer's
+The forward keeps every activation NHWC and issues, per layer, one wgmma implicit-GEMM convolution with the layer's
 elementwise tail fused in the epilogue:
   encoder convs            bias + LeakyReLU(0.2)                       (model/vtoonify.py:160-176)
   VToonifyResBlock         conv2: bias + LeakyReLU, (out + x)/sqrt(2)   (:92-104)

@@ -51,8 +51,7 @@ struct TcArgs {
   int8_t step_view[VT_MAX_TAPS], step_vx[VT_MAX_TAPS], step_vy[VT_MAX_TAPS];
   int16_t step_w[VT_MAX_TAPS];
   int step_aoff[VT_MAX_TAPS];                  // halo mode: byte offset of the tap's first row inside the halo box
-  int mt, n_phase;                             // mt accumulators (M tiles) of block_n columns per work item; n_phase: the N
-                                               // dimension is phase-major [n_phase][Cout] (folded up-conv), else 1
+  int n_phase;                                 // the N dimension is phase-major [n_phase][Cout] (folded up-conv), else 1
   int tgroup;                                  // taps per weight TMA box / pipeline step (consecutive slabs)
   int halo, halo_x0, halo_y0, halo_w;   // halo staging; x0/y0/w describe view 0's box (stride 1: the only one)
   // halo boxes of one K chunk: stride 1 has one, stride 2 one per parity view in use (each with its own extent and pitch)
@@ -79,13 +78,10 @@ struct TcArgs {
   int64_t sc_sb, sc_sy, sc_sx;
   int in_w, in_h;            // kernel-space input extents
   int mma_n;                 // N of one MMA: block_n, or 2*block_n in the N-stacked bf16x3 form
-  int nstack;                // bf16x3, Cout == 32: weight rows [w_hi|w_hi] x32 then [w_lo|w_lo] x32 -> 4 MMAs per tap, halves summed in the epilogue
   int m_major;               // work-item order: the N tiles of one pixel tile are neighbours (run on neighbouring SMs at the same
                              // time, so the second read of the activations hits L2) instead of N-tile-major
   float* stats_ws;           // optional instance-norm partial sums of the OUTPUT: [chunk][B][Cout][2] (sum, sum of squares), one chunk per
                              // (pixel tile, consumer warp); finalised by vt_instnorm_finalize_f32
-  int bf16x3;                // operands split into bf16 hi/lo in shared memory, 3 MMA products (fp32-class accuracy)
-  int fmt;                   // split-operand format: 0 = bf16 hi/lo, 1 = fp16 hi/lo
   float acc_scale;           // accumulators are multiplied by this first (undoes the power-of-two weight scale of the fp16 split)
 };
 
@@ -95,10 +91,33 @@ constexpr int CONSUMERS = 2;
 // wgmma.wait_group covers the executing warp's share of a warpgroup MMA only: every consumer warp releases a stage it has read
 constexpr int RELEASE_ARRIVALS = CONSUMERS * 4;
 
+// Operand mode of the MMAs, a template parameter of the kernel together with N and the M tiles per work item: every tap step
+// is then straight-line code (fence, the MMAs of all M tiles, commit) and compiles to one hardware wgmma group.  Runtime
+// control flow between the fence and the commit makes ptxas split the step into several groups and close it with a
+// placeholder group, so that waiting for "all but one" group waits for the step's own MMAs and drains the tensor pipe.
+enum TcOp : int {
+  OP_TF32 = 0,          // fp32 operands read as TF32: 4 MMAs m64nNk8 per 32-channel chunk
+  OP_BF16 = 1,          // bf16 hi/lo split operands, 3 products: 6 MMAs m64nNk16
+  OP_F16 = 2,           // fp16 hi/lo split operands (split_fmt = 1), 3 products
+  OP_BF16_NSTACK = 3,   // bf16 split, Cout == 32: weight rows [w_hi|w_hi] x32 then [w_lo|w_lo] x32 -> 4 MMAs of N = 64, halves
+                        // summed in the epilogue
+};
+
+template <int NW, bool F16>
+__device__ __forceinline__ void wgmma_split(float* acc, uint64_t a, uint64_t b, uint32_t accumulate) {
+  if constexpr (NW == 32) {
+    if constexpr (F16) wgmma_f16_n32(acc, a, b, accumulate); else wgmma_bf16_n32(acc, a, b, accumulate);
+  } else if constexpr (NW == 64) {
+    if constexpr (F16) wgmma_f16_n64(acc, a, b, accumulate); else wgmma_bf16_n64(acc, a, b, accumulate);
+  } else {
+    if constexpr (F16) wgmma_f16_n128(acc, a, b, accumulate); else wgmma_bf16_n128(acc, a, b, accumulate);
+  }
+}
+
 // one K step of one accumulator: the products of a 32-channel chunk (4 tf32 MMAs, or the split-operand MMAs)
-template <int NW>
-__device__ __forceinline__ void mma_step(float* acc, uint64_t adesc, uint64_t bdesc, uint32_t first, int bf16x3, int fmt, int nstack) {
-  if (!bf16x3) {
+template <int NW, int OP>
+__device__ __forceinline__ void mma_step(float* acc, uint64_t adesc, uint64_t bdesc, uint32_t first) {
+  if constexpr (OP == OP_TF32) {
     if constexpr (NW == 32) {
       wgmma_tf32_n32(acc, adesc, bdesc, first ^ 1u); wgmma_tf32_n32(acc, adesc + 2, bdesc + 2, 1);
       wgmma_tf32_n32(acc, adesc + 4, bdesc + 4, 1); wgmma_tf32_n32(acc, adesc + 6, bdesc + 6, 1);
@@ -109,34 +128,26 @@ __device__ __forceinline__ void mma_step(float* acc, uint64_t adesc, uint64_t bd
       wgmma_tf32_n128(acc, adesc, bdesc, first ^ 1u); wgmma_tf32_n128(acc, adesc + 2, bdesc + 2, 1);
       wgmma_tf32_n128(acc, adesc + 4, bdesc + 4, 1); wgmma_tf32_n128(acc, adesc + 6, bdesc + 6, 1);
     }
-    return;
-  }
-  // The A row is [a_hi(32)|a_lo(32)] and the B row [w_hi(32)|w_lo(32)] 16-bit; +2 on a descriptor = +32 B = 16 elements of K.
-  //   nstack:  [a_hi|a_lo] (K = 64) x rows [w_hi|w_hi] (columns 0..31) and [w_lo|w_lo] (columns 32..63): all four products
-  //   else:    a*w ~= a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the dropped a_lo*w_lo term is ~2^-18 relative)
-  const int ao[6] = {0, 2, 4, 6, 0, 2};
-  const int bo[6] = {0, 2, 0, 2, 4, 6};
-  const int n = nstack ? 4 : 6;
-#define VT_SPLIT_MMA(FN)                                                                   \
-  for (int i = 0; i < 6; ++i) {                                                            \
-    if (i >= n) break;                                                                     \
-    const uint64_t a_ = adesc + (uint64_t)ao[i], b_ = bdesc + (uint64_t)(nstack ? ao[i] : bo[i]); \
-    FN(acc, a_, b_, i == 0 ? (first ^ 1u) : 1u);                                           \
-  }
-  if constexpr (NW == 32) {
-    if (fmt) { VT_SPLIT_MMA(wgmma_f16_n32) } else { VT_SPLIT_MMA(wgmma_bf16_n32) }
-  } else if constexpr (NW == 64) {
-    if (fmt) { VT_SPLIT_MMA(wgmma_f16_n64) } else { VT_SPLIT_MMA(wgmma_bf16_n64) }
   } else {
-    if (fmt) { VT_SPLIT_MMA(wgmma_f16_n128) } else { VT_SPLIT_MMA(wgmma_bf16_n128) }
+    // The A row is [a_hi(32)|a_lo(32)] and the B row [w_hi(32)|w_lo(32)] 16-bit; +2 on a descriptor = +32 B = 16 elements of K.
+    //   nstack:  [a_hi|a_lo] (K = 64) x rows [w_hi|w_hi] (columns 0..31) and [w_lo|w_lo] (columns 32..63): all four products
+    //   else:    a*w ~= a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the dropped a_lo*w_lo term is ~2^-18 relative)
+    constexpr bool nstack = OP == OP_BF16_NSTACK;
+    constexpr int ao[6] = {0, 2, 4, 6, 0, 2};
+    constexpr int bo[6] = {0, 2, 0, 2, 4, 6};
+#pragma unroll
+    for (int i = 0; i < (nstack ? 4 : 6); ++i)
+      wgmma_split<NW, OP == OP_F16>(acc, adesc + (uint64_t)ao[i], bdesc + (uint64_t)(nstack ? ao[i] : bo[i]), i == 0 ? (first ^ 1u) : 1u);
   }
-#undef VT_SPLIT_MMA
 }
 
-template <int NW>
+// NW: MMA N (accumulator columns per M tile); MT: M tiles (accumulators) per work item; OP: operand mode (TcOp)
+template <int NW, int MT, int OP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcArgs p) {
-  constexpr int MTMAX = (MAX_ACC_COLS / NW) < 4 ? (MAX_ACC_COLS / NW) : 4;
+  static_assert(MT * NW <= MAX_ACC_COLS && (MT == 1 || MT == 2 || MT == 4), "accumulators of one work item exceed the register plan");
+  static_assert(OP != OP_BF16_NSTACK || NW == 64, "the N-stacked form is the Cout == 32 layer at MMA N = 64");
+  constexpr bool SPLIT = OP != OP_TF32;   // operands split into 16-bit hi/lo rows in shared memory by the transform warps
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -168,7 +179,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
 
   const int m_tiles = p.B * p.tiles_y * p.tiles_x;
   const int tiles_per_img = p.tiles_y * p.tiles_x;
-  const int item_w = TILE_W * p.mt;   // a work item covers item_w x TILE_H output pixels
+  constexpr int item_w = TILE_W * MT;   // a work item covers item_w x TILE_H output pixels
 
   if (wg == 0) {
     if (warp == 0) {
@@ -212,9 +223,9 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
                 mbar_wait(b_empty(b_st), b_par ^ 1);
                 if (elect_one()) {
                   // bf16x3: the weight row of a 32-channel chunk is one 128-byte 16-bit row [w_hi(32) | w_lo(32)]
-                  const int wc = p.bf16x3 ? (p.coff[s] + c0) * 2 : p.coff[s] + c0;
+                  const int wc = SPLIT ? (p.coff[s] + c0) * 2 : p.coff[s] + c0;
                   mbar_arrive_expect_tx(b_full(b_st), (uint32_t)p.b_tx_bytes);
-                  tma_load_4d(b_base + b_st * p.b_stage_bytes, &p.w_map, b_full(b_st), wc, p.nstack ? 0 : n0, p.step_w[j], wb);
+                  tma_load_4d(b_base + b_st * p.b_stage_bytes, &p.w_map, b_full(b_st), wc, OP == OP_BF16_NSTACK ? 0 : n0, p.step_w[j], wb);
                 }
                 __syncwarp();
                 if (++b_st == p.b_stages) { b_st = 0; b_par ^= 1; }
@@ -224,7 +235,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
           }
         }
       }
-    } else if (p.bf16x3) {
+    } else if constexpr (SPLIT) {
       // ================= operand transform (bf16x3): fp32 rows -> [hi(32) | lo(32)] 16-bit rows, in place =================
       // A 32-channel fp32 row (128 B) becomes the K = 64 row [a_hi | a_lo] with a_hi = bf16(a), a_lo = bf16(a - a_hi);
       // 16-byte chunk j of the row lives at physical chunk j ^ ((addr >> 7) & 7) (SWIZZLE_128B as TMA wrote it, kept for the MMA).
@@ -276,7 +287,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
                   }
                 }
                 uint32_t hi[16], lo[16];
-                if (p.fmt) {
+                if constexpr (OP == OP_F16) {
 #pragma unroll
                   for (int i = 0; i < 16; ++i) split_f16x2(f[2 * i], f[2 * i + 1], hi[i], lo[i]);
                 } else {
@@ -312,9 +323,9 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
     const int tw_ = (threadIdx.x & 127) >> 5;   // warp inside the warpgroup: accumulator rows [16 tw_, 16 tw_ + 16)
     const bool leader = lane == 0;   // one arrival per consumer warp
     const int qd = lane & 3;                    // column pair inside each 8-column group
-    float acc[MTMAX][NW / 2];
+    float acc[MT][NW / 2];
 #pragma unroll
-    for (int g = 0; g < MTMAX; ++g)
+    for (int g = 0; g < MT; ++g)
 #pragma unroll
       for (int i = 0; i < NW / 2; ++i) acc[g][i] = 0.f;
     const float nw = (p.noise && p.noise_w) ? *p.noise_w : 0.f;
@@ -330,10 +341,10 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
       int rel_a = -1, rel_b = -1;   // stages the previous (still in flight) wgmma group reads, released once it has completed
       for (int s = 0; s < p.n_src; ++s) {
         for (int kc = 0; kc < p.kchunks[s]; ++kc) {
-          if (p.halo) mbar_wait(p.bf16x3 ? a_ready(a_st) : a_full(a_st), a_par);
+          if (p.halo) mbar_wait(SPLIT ? a_ready(a_st) : a_full(a_st), a_par);
           int gj = 0;
           for (int j = 0; j < p.n_steps; ++j) {
-            if (!p.halo) mbar_wait(p.bf16x3 ? a_ready(a_st) : a_full(a_st), a_par);
+            if (!p.halo) mbar_wait(SPLIT ? a_ready(a_st) : a_full(a_st), a_par);
             if (gj == 0) mbar_wait(b_full(b_st), b_par);
             uint32_t a_addr = a_base + a_st * p.a_stage_bytes;
             uint32_t sbo = 1024;
@@ -348,11 +359,9 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
             const bool last_of_group = (gj == p.tgroup - 1);
             wgmma_fence();
 #pragma unroll
-            for (int g = 0; g < MTMAX; ++g) {
-              if (g < p.mt) {
-                const uint64_t adesc = make_smem_desc_sw128(a_addr + (uint32_t)(g * TILE_W * 128), sbo);
-                mma_step<NW>(acc[g], adesc, bdesc, first, p.bf16x3, p.fmt, p.nstack);
-              }
+            for (int g = 0; g < MT; ++g) {
+              const uint64_t adesc = make_smem_desc_sw128(a_addr + (uint32_t)(g * TILE_W * 128), sbo);
+              mma_step<NW, OP>(acc[g], adesc, bdesc, first);
             }
             wgmma_commit();
             wgmma_wait<1>();   // this warp's share of the group before this one has completed: its stages may be refilled
@@ -370,7 +379,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
       }
       wgmma_wait<0>();
 #pragma unroll
-      for (int g = 0; g < MTMAX; ++g) wgmma_pin<NW / 2>(acc[g]);
+      for (int g = 0; g < MT; ++g) wgmma_pin<NW / 2>(acc[g]);
       if (leader) {
         if (rel_a >= 0) mbar_arrive(a_empty(rel_a));
         if (rel_b >= 0) mbar_arrive(b_empty(rel_b));
@@ -383,8 +392,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
       const int ph0 = n0 / p.Cout, nb0 = n0 - ph0 * p.Cout;
       const int nchunks = p.block_n / 32;
 #pragma unroll
-      for (int g = 0; g < MTMAX; ++g) {
-        if (g >= p.mt) break;
+      for (int g = 0; g < MT; ++g) {
         int oy[2], ox[2];
         bool in_img[2];
         int64_t off0[2], pix0[2];
@@ -416,7 +424,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
               for (int e = 0; e < 2; ++e) {
                 const int i = 16 * j + 4 * k + 2 * h + e;
                 float x = acc[g][i];
-                if (NW == 64 && p.nstack) x += acc[g][(i + 16) % (NW / 2)];   // second column half: the w_lo products
+                if constexpr (OP == OP_BF16_NSTACK) x += acc[g][(i + 16) % (NW / 2)];   // second column half: the w_lo products
                 v[h][k][e] = x * p.acc_scale;
               }
 #pragma unroll
@@ -459,7 +467,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
           if (p.stats_ws) {
             // AdaptiveInstanceNorm statistics of the tensor this launch writes (model/dualstylegan.py:10-21): per channel, the
             // warp's 16 pixels summed in a fixed butterfly order (no atomics), pixels outside the image masked
-            const int kchunk = ((rem * p.mt + g) * STATS_WARPS) + c * 4 + tw_;
+            const int kchunk = ((rem * MT + g) * STATS_WARPS) + c * 4 + tw_;
             float2* wsp = reinterpret_cast<float2*>(p.stats_ws) + ((int64_t)kchunk * p.B + b) * p.Cout + nb + 2 * qd;
 #pragma unroll
             for (int k = 0; k < 4; ++k)
@@ -525,6 +533,20 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
     }
   }
 }
+
+// The instantiations conv_tc_run can select: every (MMA N, M tiles) with MT * NW <= MAX_ACC_COLS in each operand mode, and the
+// N-stacked form only at N = 64 (Cout == 32).
+struct TcKernel {
+  int nw, mt, op;
+  void (*fn)(TcArgs);
+};
+#define VT_TC_OPS(NW, MT) {NW, MT, OP_TF32, conv_tc_kernel<NW, MT, OP_TF32>}, {NW, MT, OP_BF16, conv_tc_kernel<NW, MT, OP_BF16>}, \
+                          {NW, MT, OP_F16, conv_tc_kernel<NW, MT, OP_F16>}
+const TcKernel kTcKernels[] = {
+    VT_TC_OPS(128, 1), VT_TC_OPS(64, 1), VT_TC_OPS(64, 2), VT_TC_OPS(32, 1), VT_TC_OPS(32, 2), VT_TC_OPS(32, 4),
+    {64, 1, OP_BF16_NSTACK, conv_tc_kernel<64, 1, OP_BF16_NSTACK>}, {64, 2, OP_BF16_NSTACK, conv_tc_kernel<64, 2, OP_BF16_NSTACK>},
+};
+#undef VT_TC_OPS
 
 }  // namespace
 
@@ -671,10 +693,10 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
   a.rgb_w = d->rgb_w; a.rgb_bias = d->rgb_bias; a.rgb_skip = d->rgb_skip; a.rgb_skip_kernel = d->rgb_skip_kernel; a.rgb_out = d->rgb_out;
   a.act = d->act; a.round_tf32 = d->round_tf32; a.slope = d->slope; a.gain = d->gain; a.alpha = d->alpha; a.beta = d->beta;
   a.B = d->B;
-  a.bf16x3 = d->weight_bf16x3 != nullptr;
-  a.fmt = (a.bf16x3 && d->split_fmt == 1) ? 1 : 0;
-  a.acc_scale = (a.bf16x3 && d->acc_scale > 0.f) ? d->acc_scale : 1.f;
-  a.nstack = (a.bf16x3 && d->bf16x3_nstack) ? 1 : 0;
+  const bool split = d->weight_bf16x3 != nullptr;
+  const bool nstack = split && d->bf16x3_nstack;
+  const int op = !split ? OP_TF32 : nstack ? OP_BF16_NSTACK : d->split_fmt == 1 ? OP_F16 : OP_BF16;
+  a.acc_scale = (split && d->acc_scale > 0.f) ? d->acc_scale : 1.f;
   a.src_scale[0] = d->src_scale[0]; a.src_scale[1] = d->src_scale[1];
   a.src_affine[0] = d->src_affine[0]; a.src_affine[1] = d->src_affine[1];
   a.src_cn[0] = d->src_c[0]; a.src_cn[1] = d->n_src > 1 ? d->src_c[1] : 0;
@@ -709,7 +731,7 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
   int bn = MAX_BLOCK_N;
   while (bn > 32 && (n_eff % bn) != 0) bn /= 2;
   VT_CHECK(n_eff % bn == 0, "conv_tc: no N tile for N=%d", n_eff);
-  const int bnm = a.nstack ? 2 * bn : bn;   // MMA N = accumulator columns = weight rows per tile
+  const int bnm = nstack ? 2 * bn : bn;  // MMA N = accumulator columns = weight rows per tile
   // halo staging: multi-tap layers (one box serves all taps) and small-N 1x1 layers (several M tiles per box and weight tile).
   // tc_mode 3: halo for stride 1 only (A/B tests)
   const bool can_halo = (g_tc_mode != 0) && (d->taps > 1 || (bn <= 64 && d->stride == 1)) && (d->stride == 1 || g_tc_mode != 3);
@@ -799,7 +821,6 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
     a.step_aoff[t] = a.hv_off[i] + ((a.step_vy[t] - vy0[v]) * hv_w[v] + (a.step_vx[t] - vx0[v])) * 128;
     a.step_sbo[t] = (uint16_t)(hv_w[v] * 128);
   }
-  a.mt = mt;
   a.block_n = bn;
   a.mma_n = bnm;
   a.n_tiles = n_eff / bn;
@@ -858,9 +879,9 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
     const uint64_t wc = (uint64_t)d->w_cstride;
     const uint64_t dims[4] = {wc, (uint64_t)n_eff, (uint64_t)d->w_taps, (uint64_t)d->wB};
     const uint64_t str[3] = {wc * 4, (uint64_t)n_eff * wc * 4, (uint64_t)d->w_taps * n_eff * wc * 4};
-    if (a.bf16x3) {   // same byte layout as the fp32 tensor: every 32-channel chunk is [w_hi(32) | w_lo(32)] bf16
+    if (split) {   // same byte layout as the fp32 tensor: every 32-channel chunk is [w_hi(32) | w_lo(32)] bf16
       VT_CHECK(((uintptr_t)d->weight_bf16x3 & 15) == 0, "conv_tc: weight_bf16x3 not 16-byte aligned");
-      const uint64_t rows = (uint64_t)n_eff * (a.nstack ? 2 : 1);   // N-stacked: 32 [w_hi|w_hi] rows then 32 [w_lo|w_lo] rows per tap
+      const uint64_t rows = (uint64_t)n_eff * (nstack ? 2 : 1);  // N-stacked: 32 [w_hi|w_hi] rows then 32 [w_lo|w_lo] rows per tap
       const uint64_t dims2[4] = {2 * wc, rows, (uint64_t)d->w_taps, (uint64_t)d->wB};
       const uint64_t str2[3] = {wc * 4, rows * wc * 4, (uint64_t)d->w_taps * rows * wc * 4};
       const uint32_t box[4] = {2 * KCH, (uint32_t)bnm, (uint32_t)a.tgroup, 1};
@@ -873,20 +894,17 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
   static std::once_flag attr_once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(attr_once, [] {
-    attr_err = cudaFuncSetAttribute(conv_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
-    if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
-    if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
+    for (const TcKernel& k : kTcKernels)
+      if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
   });
   VT_CHECK(attr_err == cudaSuccess, "conv_tc: cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err));
+  const TcKernel* kern = nullptr;
+  for (const TcKernel& k : kTcKernels)
+    if (k.nw == bnm && k.mt == mt && k.op == op) kern = &k;
+  if (!kern) return vt_set_error("conv_tc: no kernel for MMA N = %d, %d M tiles, operand mode %d", bnm, mt, op);
   int grid = vt_num_sms();
   if (grid > a.total_tiles) grid = a.total_tiles;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (bnm) {
-    case 32: conv_tc_kernel<32><<<grid, TC_THREADS, smem_bytes, st>>>(a); break;
-    case 64: conv_tc_kernel<64><<<grid, TC_THREADS, smem_bytes, st>>>(a); break;
-    case 128: conv_tc_kernel<128><<<grid, TC_THREADS, smem_bytes, st>>>(a); break;
-    default: return vt_set_error("conv_tc: no kernel for MMA N = %d", bnm);
-  }
+  kern->fn<<<grid, TC_THREADS, smem_bytes, (cudaStream_t)stream>>>(a);
   VT_LAUNCH_CHECK();
   return 0;
 }

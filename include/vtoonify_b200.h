@@ -15,6 +15,8 @@
  *                              model/stylegan/op/fused_bias_act.cpp:18-32, fused_bias_act_kernel.cu:18-105
  *   vt_conv2d_*             <- conv2d_gradfix.conv2d / conv_transpose2d (cuDNN via F.conv2d)
  *                              model/stylegan/op/conv2d_gradfix.py:22-75, and nn.Conv2d at model/vtoonify.py:96-97,111-113,162-182,195-198
+ *   vt_conv2d_wgrad         <- the weight gradient of conv2d_gradfix's backward (cudnn_convolution_backward_weight),
+ *                              model/stylegan/op/conv2d_gradfix.py:104-227
  *   vt_modulate_weights_f32 <- ModulatedConv2d weight modulation/demodulation, model/stylegan/model.py:259-267
  *   vt_linear_f32           <- EqualLinear.forward (F.linear [+ fused_leaky_relu]), model/stylegan/model.py:153-162
  *   vt_instnorm_stats_nhwc / vt_adain_apply_nhwc <- AdaptiveInstanceNorm.forward, model/dualstylegan.py:16-21
@@ -211,6 +213,38 @@ int vt_conv2d_rs_supported(const vt_conv_desc* d);
  * beyond fp32 rounding of the instance-norm partial sums (tests/test_gpu_conv.py);
  * returns the previous value (-1 for an unknown key) */
 int vt_set_option(const char* key, int value);
+
+/* ---- weight gradient of a convolution (conv2d_gradfix backward, model/stylegan/op/conv2d_gradfix.py:104-227) ---------------
+ * One reduction over pixels covers both ops:
+ *   out[m][n][t] = sum over samples b and pixels p of the A grid of  A[b, p, m] * S[b, stride*p + (tap_dy[t], tap_dx[t]), n]
+ * with S = 0 outside its image.
+ *   conv2d:           A = grad_output (M = Cout), S = input (N = Cin), tap t = ky*kw+kx at (ky*dil - pad_y, kx*dil - pad_x)
+ *   conv_transpose2d: A = input (M = Cin), S = grad_output (N = Cout), same tap offsets
+ * so `out` is the PyTorch weight layout [M][N][kh][kw] (per_sample: [B*M][N][kh][kw], the weight gradient of the groups = batch
+ * form of ModulatedConv2d, model/stylegan/model.py:273-304).  wgmma with operands split into bf16 hi + lo and three products
+ * per algorithmic product (fp32 accumulate): the accuracy class of the forward kernel's bf16x3 mode, whatever the precision
+ * setting.  The pixel reduction is split across CTAs only when the output has too few tiles to fill the GPU; the split count
+ * depends on the descriptor alone and the partial results are added in index order (no atomics): results are bit-reproducible. */
+typedef struct vt_conv_wgrad_desc {
+  int32_t struct_size;          /* sizeof(vt_conv_wgrad_desc), ABI check                                              */
+  int32_t B;                    /* samples                                                                            */
+  int32_t per_sample;           /* 0: sum over samples, out [M][N][taps]; 1: one result per sample, out [B*M][N][taps] */
+  int32_t stride;               /* 1 or 2                                                                             */
+  const float* a;               /* NHWC [B, a_h, a_w, a_cstride]; channels [M, a_cstride) must be zero (padding)     */
+  int32_t a_h, a_w, M, a_cstride;   /* a_cstride % 32 == 0                                                            */
+  const float* s;               /* NHWC [B, s_h, s_w, s_cstride]                                                      */
+  int32_t s_h, s_w, N, s_cstride;   /* s_cstride % 32 == 0                                                            */
+  int32_t taps;                 /* 1 .. VT_MAX_TAPS                                                                   */
+  int32_t tap_dy[VT_MAX_TAPS];
+  int32_t tap_dx[VT_MAX_TAPS];
+  float*  out;
+  float*  ws;                   /* workspace of vt_conv2d_wgrad_ws_floats(desc) floats (NULL when that is 0)          */
+  int64_t ws_floats;
+} vt_conv_wgrad_desc;
+/* workspace floats vt_conv2d_wgrad needs for this descriptor (0 when the reduction is not split); host only: plans without
+ * touching the GPU.  -1 + vt_last_error() for a descriptor vt_conv2d_wgrad rejects. */
+int64_t vt_conv2d_wgrad_ws_floats(const vt_conv_wgrad_desc* d);
+int vt_conv2d_wgrad(const vt_conv_wgrad_desc* d, void* stream);
 
 /* ---- small-N conv (Cout <= 4): planar output, optional planar extra source + skip upsample */
 typedef struct vt_smalln_desc {

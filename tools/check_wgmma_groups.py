@@ -1,18 +1,19 @@
 """Check that every tap step of the tensor-core convolution compiles to one wgmma commit group.
 
-    python tools/check_wgmma_groups.py [--lib vtoonify_b200/lib/libvtoonify_b200.so] [--log build.log]
+    python tools/check_wgmma_groups.py [--lib vtoonify_b200/lib/libvtoonify_b200.so] [--log build.log] [--kernel conv_wgrad_kernel]
 
 conv_tc_kernel keeps one wgmma group in flight while it waits for the next pipeline stage. That only works when ptxas keeps
 each step's MMAs in one hardware group. When it cannot (runtime control flow between wgmma.fence and wgmma.commit_group, or
 a printf anywhere in the kernel), it splits the step and closes it with a placeholder HGMMA. The wait for "all but one
 group" then waits for the step's own MMAs, and the tensor pipe drains at every step. Results are still correct; only the
-speed drops. The symptoms in the SASS (cuobjdump -sass of the built library), for every conv_tc_kernel instantiation:
+speed drops. The symptoms in the SASS (cuobjdump -sass of the built library), for every instantiation of the kernel (--kernel,
+default conv_tc_kernel; the weight-gradient kernel conv_wgrad_kernel follows the same one-group-per-step rule):
 
   * a placeholder HGMMA, which writes RZ (`HGMMA.64x8x16.F16 RZ, gdesc[URZ], RZ, !UPT, gsb0`);
   * an HGMMA that closes a group (`gsb0`) and is followed by another HGMMA before any `WARPGROUP.DEPBAR` (wait).
 
 With --log, a build log of `VT_PTXAS_V=1 vtoonify_b200/csrc/build.sh` is also checked for ptxas' C7519 notice
-("warpgroup.arrive is injected ...") on conv_tc_kernel. Exit status 0 when every check passes, 1 otherwise.
+("warpgroup.arrive is injected ...") on that kernel. Exit status 0 when every check passes, 1 otherwise.
 """
 import argparse
 import os
@@ -39,18 +40,20 @@ def find_cuobjdump():
     return None
 
 
-def short_name(mangled):
-    m = re.search(KERNEL + r"ILi(\d+)ELi(\d+)ELi(\d+)E", mangled)
-    return f"{KERNEL}<{m.group(1)}, {m.group(2)}, {m.group(3)}>" if m else mangled
+def short_name(mangled, kernel=KERNEL):
+    m = re.search(kernel + r"I((?:Li\d+E)+)E", mangled)
+    if not m:
+        return mangled
+    return kernel + "<" + ", ".join(re.findall(r"Li(\d+)E", m.group(1))) + ">"
 
 
-def kernel_sass(sass_text):
-    """{function name: [instruction text]} for every conv_tc_kernel instantiation in a cuobjdump -sass listing."""
+def kernel_sass(sass_text, kernel=KERNEL):
+    """{function name: [instruction text]} for every instantiation of `kernel` in a cuobjdump -sass listing."""
     funcs, cur = {}, None
     for line in sass_text.splitlines():
         if "Function :" in line:
             name = line.split("Function :", 1)[1].strip()
-            cur = funcs.setdefault(name, []) if KERNEL in name else None
+            cur = funcs.setdefault(name, []) if kernel in name else None
         elif cur is not None:
             m = _INSN.search(line)
             if m:
@@ -75,14 +78,15 @@ def check_groups(insns):
     return n_mma, n_groups, problems
 
 
-def check_log(log_text):
-    return [line.strip() for line in log_text.splitlines() if "C7519" in line and KERNEL in line]
+def check_log(log_text, kernel=KERNEL):
+    return [line.strip() for line in log_text.splitlines() if "C7519" in line and kernel in line]
 
 
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--lib", default=DEFAULT_LIB, help="the built shared library")
     ap.add_argument("--log", default=None, help="build log of VT_PTXAS_V=1 vtoonify_b200/csrc/build.sh")
+    ap.add_argument("--kernel", default=KERNEL, help="kernel (template) name whose instantiations are checked")
     args = ap.parse_args(argv)
 
     tool = find_cuobjdump()
@@ -93,22 +97,22 @@ def main(argv=None):
         print(f"check_wgmma_groups: {args.lib} does not exist (build it first)", file=sys.stderr)
         return 2
     sass = subprocess.run([tool, "-sass", args.lib], capture_output=True, text=True, check=True).stdout
-    funcs = kernel_sass(sass)
+    funcs = kernel_sass(sass, args.kernel)
     failed = False
     if not funcs:
-        print(f"FAIL: no {KERNEL} in {args.lib}")
+        print(f"FAIL: no {args.kernel} in {args.lib}")
         failed = True
-    for name in sorted(funcs, key=short_name):
+    for name in sorted(funcs, key=lambda n: short_name(n, args.kernel)):
         n_mma, n_groups, problems = check_groups(funcs[name])
         if n_mma == 0:
             problems.append("no HGMMA instructions")
-        print(f"{'FAIL' if problems else 'ok  '} {short_name(name)}: {n_mma} HGMMA, {n_groups} groups")
+        print(f"{'FAIL' if problems else 'ok  '} {short_name(name, args.kernel)}: {n_mma} HGMMA, {n_groups} groups")
         for p in problems:
             print(f"       {p}")
         failed = failed or bool(problems)
     if args.log:
         with open(args.log) as f:
-            notices = check_log(f.read())
+            notices = check_log(f.read(), args.kernel)
         for line in notices:
             print(f"FAIL ptxas: {line}")
         failed = failed or bool(notices)

@@ -41,6 +41,16 @@ class ConvDesc(Structure):
     ]
 
 
+class ConvWgradDesc(Structure):
+    _fields_ = [
+        ("struct_size", c_int32), ("B", c_int32), ("per_sample", c_int32), ("stride", c_int32),
+        ("a", c_void_p), ("a_h", c_int32), ("a_w", c_int32), ("M", c_int32), ("a_cstride", c_int32),
+        ("s", c_void_p), ("s_h", c_int32), ("s_w", c_int32), ("N", c_int32), ("s_cstride", c_int32),
+        ("taps", c_int32), ("tap_dy", c_int32 * VT_MAX_TAPS), ("tap_dx", c_int32 * VT_MAX_TAPS),
+        ("out", c_void_p), ("ws", c_void_p), ("ws_floats", c_int64),
+    ]
+
+
 class SmallNDesc(Structure):
     _fields_ = [
         ("struct_size", c_int32), ("n_planar", c_int32),
@@ -85,6 +95,8 @@ SYMBOLS = {
     "vt_conv2d_rs": (c_int, [POINTER(ConvDesc), c_float, _P]),
     "vt_conv2d_rs_supported": (c_int, [POINTER(ConvDesc)]),
     "vt_set_option": (c_int, [c_char_p, c_int]),
+    "vt_conv2d_wgrad_ws_floats": (c_int64, [POINTER(ConvWgradDesc)]),
+    "vt_conv2d_wgrad": (c_int, [POINTER(ConvWgradDesc), _P]),
     "vt_smalln_conv_f32": (c_int, [POINTER(SmallNDesc), _P]),
     "vt_affine_fold_weights_f32": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),
     "vt_fir_nhwc_f32": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, c_int,

@@ -618,6 +618,39 @@ def conv_transpose2d_s2_k3_nhwc(x: torch.Tensor, weight: torch.Tensor, precision
     return out
 
 
+def conv_wgrad_nhwc(a: torch.Tensor, s: torch.Tensor, M: int, N: int, taps, stride: int, per_sample: bool) -> torch.Tensor:
+    """Weight gradient ``out[m, n, t] = sum_{b, p} a[b, p, m] * s[b, stride * p + (dy_t, dx_t), n]`` (zero outside ``s``) on the
+    wgmma weight-gradient kernel (bf16x3 arithmetic whatever :func:`set_precision` says).  ``a``, ``s``: contiguous NHWC with channel
+    strides that are multiples of 32 (:func:`to_nhwc` with ``c_pad``); ``taps``: [(dy, dx)].  Returns ``[nb * M, N, len(taps)]``,
+    nb = B when ``per_sample`` else 1.  Deterministic: the same inputs give bit-identical results."""
+    _req_cuda(a, s)
+    B, Ha, Wa, ca = a.shape
+    Bs, Hs, Ws, cs = s.shape
+    if Bs != B or not a.is_contiguous() or not s.is_contiguous():
+        raise _lib.VtError("conv_wgrad_nhwc: a and s must be contiguous NHWC tensors with the same batch")
+    d = _lib.ConvWgradDesc()
+    d.struct_size = _lib.ctypes.sizeof(_lib.ConvWgradDesc)
+    d.B, d.per_sample, d.stride = B, int(per_sample), stride
+    d.a, d.a_h, d.a_w, d.M, d.a_cstride = a.data_ptr(), Ha, Wa, M, ca
+    d.s, d.s_h, d.s_w, d.N, d.s_cstride = s.data_ptr(), Hs, Ws, N, cs
+    d.taps = len(taps)
+    if d.taps > _lib.VT_MAX_TAPS:
+        raise _lib.VtError(f"conv_wgrad_nhwc: at most {_lib.VT_MAX_TAPS} taps")
+    for t, (dy, dx) in enumerate(taps):
+        d.tap_dy[t], d.tap_dx[t] = dy, dx
+    lib = _lib.load()
+    n_ws = lib.vt_conv2d_wgrad_ws_floats(d)
+    if n_ws < 0:
+        check(1)
+    out = torch.empty(((B if per_sample else 1) * M, N, len(taps)), device=a.device, dtype=torch.float32)
+    ws = torch.empty((n_ws,), device=a.device, dtype=torch.float32) if n_ws > 0 else None
+    d.out = out.data_ptr()
+    if ws is not None:
+        d.ws, d.ws_floats = ws.data_ptr(), n_ws
+    check(lib.vt_conv2d_wgrad(d, _stream()))
+    return out
+
+
 def fold_upconv_weights(w: torch.Tensor, blur_kernel: torch.Tensor) -> torch.Tensor:
     """[wB, 9, Cout, cpad] modulated weights (un-rounded) + 4x4 blur -> [wB, 9, 4*Cout, cpad]: per tap the 4 phase kernels
     stacked along the GEMM N dimension."""

@@ -32,6 +32,9 @@ extern int g_upfirdn_tiled;
 extern int g_smalln_is;
 extern int g_fir4;
 extern int g_instnorm_chunks;
+extern int g_rs_kernel;
+int vt_conv_rs_takes(const vt_conv_desc* d);
+int vt_conv_rs_run(const vt_conv_desc* d, void* stream);
 
 namespace {
 
@@ -495,38 +498,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             if (qd != 0 || !in_img[h]) continue;
-            const int py = oy[h], px = ox[h];
-            // + bias + Upsample(skip): upfirdn2d(up=2, pad=(2,1), 4x4 kernel) touches exactly 2x2 skip pixels per output
-            // pixel (taps with (y-2+ky) even).  Branch-free: clamped addresses + validity masks so the 12 loads issue together.
-            float o[3] = {rgb[h][0] + __ldg(p.rgb_bias), rgb[h][1] + __ldg(p.rgb_bias + 1), rgb[h][2] + __ldg(p.rgb_bias + 2)};
-            const int64_t HW = (int64_t)p.Ho * p.Wo;
-            if (p.rgb_skip) {
-              const int hs = p.Ho >> 1, ws = p.Wo >> 1;
-              const int ky0 = (py - 2) & 1, kx0 = (px - 2) & 1;
-              const int iy0 = (py - 2 + ky0) >> 1, ix0 = (px - 2 + kx0) >> 1;        // second tap is +1
-              const float my0 = iy0 >= 0 ? 1.f : 0.f, my1 = (iy0 + 1) < hs ? 1.f : 0.f;
-              const float mx0 = ix0 >= 0 ? 1.f : 0.f, mx1 = (ix0 + 1) < ws ? 1.f : 0.f;
-              const int cy0 = iy0 < 0 ? 0 : iy0, cy1 = (iy0 + 1) < hs ? iy0 + 1 : hs - 1;
-              const int cx0 = ix0 < 0 ? 0 : ix0, cx1 = (ix0 + 1) < ws ? ix0 + 1 : ws - 1;
-              // flipped-kernel weights of the 4 taps (ky in {ky0, ky0+2}, kx in {kx0, kx0+2})
-              const float* kk = p.rgb_skip_kernel;
-              const float w00 = __ldg(kk + (3 - ky0) * 4 + (3 - kx0)) * my0 * mx0;
-              const float w01 = __ldg(kk + (3 - ky0) * 4 + (1 - kx0)) * my0 * mx1;
-              const float w10 = __ldg(kk + (1 - ky0) * 4 + (3 - kx0)) * my1 * mx0;
-              const float w11 = __ldg(kk + (1 - ky0) * 4 + (1 - kx0)) * my1 * mx1;
-#pragma unroll
-              for (int cc = 0; cc < 3; ++cc) {
-                const float* sp = p.rgb_skip + ((int64_t)b * 3 + cc) * (int64_t)hs * ws;
-                // same accumulation order as the reference loop (ky outer, kx inner)
-                float u = __ldg(sp + (int64_t)cy0 * ws + cx0) * w00;
-                u = fmaf(__ldg(sp + (int64_t)cy0 * ws + cx1), w01, u);
-                u = fmaf(__ldg(sp + (int64_t)cy1 * ws + cx0), w10, u);
-                u = fmaf(__ldg(sp + (int64_t)cy1 * ws + cx1), w11, u);
-                o[cc] += u;
-              }
-            }
-#pragma unroll
-            for (int cc = 0; cc < 3; ++cc) p.rgb_out[((int64_t)b * 3 + cc) * HW + (int64_t)py * p.Wo + px] = o[cc];
+            torgb_store(p.rgb_bias, p.rgb_skip, p.rgb_skip_kernel, p.rgb_out, rgb[h], b, oy[h], ox[h], p.Ho, p.Wo);
           }
         }
       }
@@ -643,6 +615,7 @@ extern "C" int vt_set_option(const char* key, int value) {
   if (key && strcmp(key, "tc_halo_pct") == 0) { int old = g_tc_halo_pct; g_tc_halo_pct = value; return old; }
   if (key && strcmp(key, "tc_m_major") == 0) { int old = g_tc_m_major; g_tc_m_major = value; return old; }
   if (key && strcmp(key, "tc_transpose") == 0) { int old = g_tc_transpose; g_tc_transpose = value; return old; }
+  if (key && strcmp(key, "rs_kernel") == 0) { int old = g_rs_kernel; g_rs_kernel = value; return old; }
   if (key && strcmp(key, "instnorm_chunks") == 0) { int old = g_instnorm_chunks; g_instnorm_chunks = value; return old; }
   if (key && strcmp(key, "fir4") == 0) { int old = g_fir4; g_fir4 = value; return old; }
   if (key && strcmp(key, "smalln_is") == 0) { int old = g_smalln_is; g_smalln_is = value; return old; }
@@ -911,8 +884,8 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
 
 extern "C" int vt_conv2d_tc_tf32(const vt_conv_desc* d, void* stream) { return conv_tc_run(d, stream, nullptr); }
 
-// Row-strip entry points: the full-resolution 3x3 / stride 1 layers with Cin, Cout in {32, 64}.  On sm_90a they run the wgmma kernel
-// above (the Blackwell build accumulated rows across input rows in tensor memory, which Hopper does not have).
+// Row-strip entry points: the full-resolution 3x3 / stride 1 layers with Cin, Cout in {32, 64}.  They run conv_rs_kernel
+// (conv_rs.cu: output channels on the MMA's M, pixels on N) when it takes the descriptor, else the kernel above.
 static bool rs_shape(const vt_conv_desc* d) {
   if (d->n_src != 1 || d->stride != 1 || d->taps != 9 || d->n_phase != 1 || d->res || d->slope_vec || !d->weight_bf16x3) return false;
   if (d->src_scale[0] || d->src_affine[0] || d->alpha != 1.f) return false;
@@ -929,6 +902,7 @@ extern "C" int vt_conv2d_rs(const vt_conv_desc* d, float acc_scale, void* stream
   VT_CHECK(d && d->struct_size == (int)sizeof(vt_conv_desc) && rs_shape(d), "conv2d_rs: not a row-strip layer (3x3, stride 1, Cin/Cout in {32, 64})");
   vt_conv_desc c = *d;
   if (acc_scale > 0.f) c.acc_scale = acc_scale;
+  if (g_rs_kernel && vt_conv_rs_takes(&c)) return vt_conv_rs_run(&c, stream);
   return conv_tc_run(&c, stream, nullptr);
 }
 

@@ -88,6 +88,63 @@ __device__ __forceinline__ void split_f16x2(float x0, float x1, uint32_t& hi, ui
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(x1 - h1), "f"(x0 - h0));
 }
 
+// Fused ToRGB, Upsample(skip) part for one output pixel (py, px) of sample b: upfirdn2d(up=2, pad=(2,1), 4x4 kernel) touches exactly
+// 2x2 skip pixels per output pixel (taps with (y-2+ky) even).  Branch-free: clamped addresses + validity masks so the 12 loads
+// issue together.  Loading (skip_taps_load) and summing (skip_taps_sum) are separate so that a kernel can issue the loads early.
+struct SkipTaps {
+  float v[3][4];   // skip values of the 4 taps per colour
+  float w[4];      // masked flipped-kernel weights of the 4 taps (ky in {ky0, ky0+2}, kx in {kx0, kx0+2})
+};
+__device__ __forceinline__ void skip_taps_load(const float* rgb_skip, const float* kk, int b, int py, int px, int Ho, int Wo, SkipTaps& s) {
+  const int hs = Ho >> 1, ws = Wo >> 1;
+  const int ky0 = (py - 2) & 1, kx0 = (px - 2) & 1;
+  const int iy0 = (py - 2 + ky0) >> 1, ix0 = (px - 2 + kx0) >> 1;        // second tap is +1
+  const float my0 = iy0 >= 0 ? 1.f : 0.f, my1 = (iy0 + 1) < hs ? 1.f : 0.f;
+  const float mx0 = ix0 >= 0 ? 1.f : 0.f, mx1 = (ix0 + 1) < ws ? 1.f : 0.f;
+  const int cy0 = iy0 < 0 ? 0 : iy0, cy1 = (iy0 + 1) < hs ? iy0 + 1 : hs - 1;
+  const int cx0 = ix0 < 0 ? 0 : ix0, cx1 = (ix0 + 1) < ws ? ix0 + 1 : ws - 1;
+  s.w[0] = __ldg(kk + (3 - ky0) * 4 + (3 - kx0)) * my0 * mx0;
+  s.w[1] = __ldg(kk + (3 - ky0) * 4 + (1 - kx0)) * my0 * mx1;
+  s.w[2] = __ldg(kk + (1 - ky0) * 4 + (3 - kx0)) * my1 * mx0;
+  s.w[3] = __ldg(kk + (1 - ky0) * 4 + (1 - kx0)) * my1 * mx1;
+#pragma unroll
+  for (int cc = 0; cc < 3; ++cc) {
+    const float* sp = rgb_skip + ((int64_t)b * 3 + cc) * (int64_t)hs * ws;
+    s.v[cc][0] = __ldg(sp + (int64_t)cy0 * ws + cx0);
+    s.v[cc][1] = __ldg(sp + (int64_t)cy0 * ws + cx1);
+    s.v[cc][2] = __ldg(sp + (int64_t)cy1 * ws + cx0);
+    s.v[cc][3] = __ldg(sp + (int64_t)cy1 * ws + cx1);
+  }
+}
+// same accumulation order as the reference loop (ky outer, kx inner)
+__device__ __forceinline__ float skip_taps_sum(const SkipTaps& s, int cc) {
+  float u = s.v[cc][0] * s.w[0];
+  u = fmaf(s.v[cc][1], s.w[1], u);
+  u = fmaf(s.v[cc][2], s.w[2], u);
+  u = fmaf(s.v[cc][3], s.w[3], u);
+  return u;
+}
+
+// Fused ToRGB, last step for one output pixel: rgb (the 1x1 modulated conv over the pixel's channels) + bias + Upsample(skip)
+// (the taps in `st`, loaded by skip_taps_load when rgb_skip is set), written to the planar [B][3][Ho][Wo] image
+__device__ __forceinline__ void torgb_store_taps(const float* rgb_bias, bool skip, const SkipTaps& st, float* rgb_out, const float rgb[3],
+                                                 int b, int py, int px, int Ho, int Wo) {
+  float o[3] = {rgb[0] + __ldg(rgb_bias), rgb[1] + __ldg(rgb_bias + 1), rgb[2] + __ldg(rgb_bias + 2)};
+  if (skip) {
+#pragma unroll
+    for (int cc = 0; cc < 3; ++cc) o[cc] += skip_taps_sum(st, cc);
+  }
+  const int64_t HW = (int64_t)Ho * Wo;
+#pragma unroll
+  for (int cc = 0; cc < 3; ++cc) rgb_out[((int64_t)b * 3 + cc) * HW + (int64_t)py * Wo + px] = o[cc];
+}
+__device__ __forceinline__ void torgb_store(const float* rgb_bias, const float* rgb_skip, const float* kk, float* rgb_out, const float rgb[3],
+                                            int b, int py, int px, int Ho, int Wo) {
+  SkipTaps st;
+  if (rgb_skip) skip_taps_load(rgb_skip, kk, b, py, px, Ho, Wo, st);
+  torgb_store_taps(rgb_bias, rgb_skip != nullptr, st, rgb_out, rgb, b, py, px, Ho, Wo);
+}
+
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

@@ -501,8 +501,11 @@ def conv2d_nhwc(srcs: Sequence[torch.Tensor], weight: torch.Tensor, taps, stride
     d.weight_bf16x3 = None
     if use_tc and prec == "bf16x3":
         # Cout == 32: the N-stacked form needs 4 instead of 6 MMA instructions per tap (and keeps all four hi/lo products) but
-        # twice the accumulator columns; off by default
-        nstack = bool(_options["bf16x3_nstack"]) and Cout == 32 and phase_offs is None
+        # twice the accumulator columns; off by default.  The row-strip kernel (conv_rs_kernel) reads exactly this form for Cout == 32
+        # (its 64 weight rows are the MMA's M), so the rs route gets it with the bf16 split; a launch that also writes instance-norm
+        # statistics is one conv_rs_kernel does not take and keeps the plain split
+        nstack = Cout == 32 and phase_offs is None and (bool(_options["bf16x3_nstack"]) or
+                                                        (rs and _options["rs_fmt"] == "bf16" and not want_stats))
         if _options["rs_fmt"] == "f16" and not nstack:
             d.weight_bf16x3 = split_weights_f16x3(weight).data_ptr()
             d.split_fmt, d.acc_scale = 1, 1.0 / F16_WEIGHT_SCALE

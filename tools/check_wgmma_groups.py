@@ -13,7 +13,13 @@ default conv_tc_kernel; the weight-gradient kernel conv_wgrad_kernel follows the
   * an HGMMA that closes a group (`gsb0`) and is followed by another HGMMA before any `WARPGROUP.DEPBAR` (wait).
 
 With --log, a build log of `VT_PTXAS_V=1 vtoonify_b200/csrc/build.sh` is also checked for ptxas' C7519 notice
-("warpgroup.arrive is injected ...") on that kernel. Exit status 0 when every check passes, 1 otherwise.
+("warpgroup.arrive is injected ...") on that kernel.
+
+An instantiation that moves registers between its warpgroups (setmaxnreg: `USETMAXREG.DEALLOC` in warpgroup 0, the producer
+and transform warps, and `USETMAXREG.TRY_ALLOC` in the two consumer warpgroups) is also checked against the register count
+the launch allocates (`cuobjdump -res-usage`): 128 * dec + 256 * inc must not exceed 384 * REG, and the instantiation must not
+spill. `setmaxnreg.inc` waits until enough registers are free, so a plan above the allocation hangs instead of failing.
+Exit status 0 when every check passes, 1 otherwise.
 """
 import argparse
 import os
@@ -78,6 +84,49 @@ def check_groups(insns):
     return n_mma, n_groups, problems
 
 
+_MAXREG = re.compile(r"USETMAXREG\.(DEALLOC|TRY_ALLOC)\.CTAPOOL\s+(?:U?P\w+\s*,\s*)?(0x[0-9a-f]+|\d+)")
+_RES = re.compile(r"Function\s+(\S+?):\s*REG:(\d+)\s+STACK:(\d+)\s+SHARED:\d+\s+LOCAL:(\d+)")
+THREADS, XFORM_THREADS, CONSUMER_THREADS = 384, 128, 256
+
+
+def maxreg_plan(insns):
+    """(dec, inc) register counts of the setmaxnreg instructions of one function; None for either that is absent."""
+    dec = inc = None
+    for ins in insns:
+        m = _MAXREG.search(ins)
+        if m:
+            v = int(m.group(2), 0)
+            if m.group(1) == "DEALLOC":
+                dec = v
+            else:
+                inc = v
+    return dec, inc
+
+
+def res_usage(text):
+    """{function name: (REG, STACK, LOCAL)} from a cuobjdump -res-usage listing."""
+    return {m.group(1): (int(m.group(2)), int(m.group(3)), int(m.group(4))) for m in _RES.finditer(text)}
+
+
+def check_regs(insns, usage):
+    """[problems] of one function's register reallocation; usage = (REG, STACK, LOCAL) or None. Empty without setmaxnreg."""
+    dec, inc = maxreg_plan(insns)
+    if dec is None and inc is None:
+        return []
+    if dec is None or inc is None:
+        return [f"setmaxnreg plan incomplete (dec {dec}, inc {inc})"]
+    if usage is None:
+        return ["no -res-usage entry for the function"]
+    reg, stack, local = usage
+    problems = []
+    if XFORM_THREADS * dec + CONSUMER_THREADS * inc > THREADS * reg:
+        problems.append(f"setmaxnreg plan {XFORM_THREADS} x {dec} + {CONSUMER_THREADS} x {inc} = "
+                        f"{XFORM_THREADS * dec + CONSUMER_THREADS * inc} registers exceeds the launch's {THREADS} x {reg} = {THREADS * reg}")
+    if stack or local:
+        problems.append(f"spills ({stack} bytes stack, {local} bytes local)")
+    return problems
+
+
 def check_log(log_text, kernel=KERNEL):
     return [line.strip() for line in log_text.splitlines() if "C7519" in line and kernel in line]
 
@@ -98,6 +147,7 @@ def main(argv=None):
         return 2
     sass = subprocess.run([tool, "-sass", args.lib], capture_output=True, text=True, check=True).stdout
     funcs = kernel_sass(sass, args.kernel)
+    usage = res_usage(subprocess.run([tool, "-res-usage", args.lib], capture_output=True, text=True, check=True).stdout)
     failed = False
     if not funcs:
         print(f"FAIL: no {args.kernel} in {args.lib}")
@@ -106,7 +156,10 @@ def main(argv=None):
         n_mma, n_groups, problems = check_groups(funcs[name])
         if n_mma == 0:
             problems.append("no HGMMA instructions")
-        print(f"{'FAIL' if problems else 'ok  '} {short_name(name, args.kernel)}: {n_mma} HGMMA, {n_groups} groups")
+        problems += check_regs(funcs[name], usage.get(name))
+        dec, inc = maxreg_plan(funcs[name])
+        regs = f", setmaxnreg {dec}/{inc} of {usage[name][0]}" if dec is not None and name in usage else ""
+        print(f"{'FAIL' if problems else 'ok  '} {short_name(name, args.kernel)}: {n_mma} HGMMA, {n_groups} groups{regs}")
         for p in problems:
             print(f"       {p}")
         failed = failed or bool(problems)

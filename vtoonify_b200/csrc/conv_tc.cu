@@ -41,8 +41,15 @@ namespace {
 constexpr int TILE_W = 8, TILE_H = 16, TILE_M = 128;
 constexpr int KCH = 32;                       // fp32 channels per K chunk = one 128-byte swizzle row
 constexpr int MAX_SMEM = 227 * 1024;
-constexpr int MAX_BLOCK_N = 128;              // largest N tile (wgmma N) of one work item
-constexpr int MAX_ACC_COLS = 128;             // accumulator columns per consumer thread group: mt * mma_n (64 registers; 128 spill)
+constexpr int MAX_BLOCK_N = 128;              // largest N tile (wgmma N) of one work item under the flat register budget
+constexpr int MAX_ACC_COLS = 128;             // accumulator columns per consumer thread group: mt * mma_n (64 registers) under the flat
+                                              // budget of 168 registers per thread; 256 columns spill there
+// The wide work item: 128 pixels x 256 output channels on m64n256k16 (bf16 split only, one M tile).  Its 256 accumulator
+// columns (128 registers) fit because warpgroup 0 (producer + transform warps) hands registers to the two consumer
+// warpgroups with setmaxnreg: 128 * WIDE_REGS_XFORM + 256 * WIDE_REGS_CONSUMER <= 384 * 168, the launch allocation.
+constexpr int WIDE_N = 256;
+constexpr int WIDE_REGS_XFORM = 88;
+constexpr int WIDE_REGS_CONSUMER = 208;
 constexpr int STATS_WARPS = 8;                // instance-norm chunks per 128-pixel tile: one per consumer warp (16 pixels)
 
 struct TcArgs {
@@ -62,6 +69,7 @@ struct TcArgs {
   uint16_t step_sbo[VT_MAX_TAPS];   // halo mode: stride (bytes) between 8-pixel row groups of the tap's box
   int a_stages, b_stages, a_stage_bytes, b_stage_bytes, a_tx_bytes, b_tx_bytes;
   int block_n, n_tiles, tiles_x, tiles_y, B, total_tiles;
+  int m_first;               // first pixel tile of this launch: a layer may run its pixel tiles as a wide and a narrow launch
   int Ho, Wo, Cout, wB, out_cpitch;
   const float* bias;
   const float* noise;
@@ -112,8 +120,11 @@ __device__ __forceinline__ void wgmma_split(float* acc, uint64_t a, uint64_t b, 
     if constexpr (F16) wgmma_f16_n32(acc, a, b, accumulate); else wgmma_bf16_n32(acc, a, b, accumulate);
   } else if constexpr (NW == 64) {
     if constexpr (F16) wgmma_f16_n64(acc, a, b, accumulate); else wgmma_bf16_n64(acc, a, b, accumulate);
-  } else {
+  } else if constexpr (NW == 128) {
     if constexpr (F16) wgmma_f16_n128(acc, a, b, accumulate); else wgmma_bf16_n128(acc, a, b, accumulate);
+  } else {
+    static_assert(NW == WIDE_N && !F16, "the 256-wide MMA exists for the bf16 split only");
+    wgmma_bf16_n256(acc, a, b, accumulate);
   }
 }
 
@@ -148,7 +159,15 @@ __device__ __forceinline__ void mma_step(float* acc, uint64_t adesc, uint64_t bd
 template <int NW, int MT, int OP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcArgs p) {
-  static_assert(MT * NW <= MAX_ACC_COLS && (MT == 1 || MT == 2 || MT == 4), "accumulators of one work item exceed the register plan");
+  // The wide item is the one instantiation that reallocates registers between the warpgroups.  Its epilogue leaves out the
+  // fused ToRGB and the tanh activation (the planner never gives it those layers): with them, the fully unrolled 8-chunk
+  // epilogue made the kernel 11.6k instructions, which no longer stay in the instruction cache, and every layer ran slower
+  // wide than 128-wide; without them it is 7.0k, the size of the 128-wide kernel.
+  constexpr bool WIDE = NW == WIDE_N;
+  static_assert((MT * NW <= MAX_ACC_COLS || (WIDE && MT == 1 && OP == OP_BF16)) && (MT == 1 || MT == 2 || MT == 4),
+                "accumulators of one work item exceed the register plan");
+  static_assert(128 * WIDE_REGS_XFORM + 256 * WIDE_REGS_CONSUMER <= TC_THREADS * ((65536 / TC_THREADS) & ~7),
+                "setmaxnreg plan exceeds the launch allocation");
   static_assert(OP != OP_BF16_NSTACK || NW == 64, "the N-stacked form is the Cout == 32 layer at MMA N = 64");
   constexpr bool SPLIT = OP != OP_TF32;   // operands split into 16-bit hi/lo rows in shared memory by the transform warps
   extern __shared__ uint8_t smem_raw[];
@@ -180,17 +199,18 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
   }
   __syncthreads();
 
-  const int m_tiles = p.B * p.tiles_y * p.tiles_x;
+  const int m_tiles = p.total_tiles / p.n_tiles;   // pixel tiles of this launch, from p.m_first on
   const int tiles_per_img = p.tiles_y * p.tiles_x;
   constexpr int item_w = TILE_W * MT;   // a work item covers item_w x TILE_H output pixels
 
   if (wg == 0) {
+    if constexpr (WIDE) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WIDE_REGS_XFORM));
     if (warp == 0) {
       // ================= TMA producer (whole warp converged; one elected lane issues) =================
       int a_st = 0, b_st = 0;
       uint32_t a_par = 0, b_par = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int n_tile = p.m_major ? tile % p.n_tiles : tile / m_tiles, m = p.m_major ? tile / p.n_tiles : tile % m_tiles;
+        const int n_tile = p.m_major ? tile % p.n_tiles : tile / m_tiles, m = p.m_first + (p.m_major ? tile / p.n_tiles : tile % m_tiles);
         const int b = m / tiles_per_img, rem = m % tiles_per_img;
         const int oy0 = (rem / p.tiles_x) * TILE_H, ox0 = (rem % p.tiles_x) * item_w;
         const int n0 = n_tile * p.block_n;
@@ -248,7 +268,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
       uint32_t a_par = 0;
       const int bw = p.halo ? p.halo_w : TILE_W;   // pixels per box row
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int m = p.m_major ? tile / p.n_tiles : tile % m_tiles;
+        const int m = p.m_first + (p.m_major ? tile / p.n_tiles : tile % m_tiles);
         const int b = m / tiles_per_img, rem = m % tiles_per_img;
         const int oy0 = (rem / p.tiles_x) * TILE_H, ox0 = (rem % p.tiles_x) * item_w;
         for (int s = 0; s < p.n_src; ++s) {
@@ -322,6 +342,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
     }
   } else {
     // ================= consumers: wgmma main loop + epilogue =================
+    if constexpr (WIDE) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WIDE_REGS_CONSUMER));
     const int c = wg - 1;                       // pixel rows [8c, 8c + 8) of the 8 x 16 tile
     const int tw_ = (threadIdx.x & 127) >> 5;   // warp inside the warpgroup: accumulator rows [16 tw_, 16 tw_ + 16)
     const bool leader = lane == 0;   // one arrival per consumer warp
@@ -336,7 +357,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
     uint32_t a_par = 0, b_par = 0;
     const uint32_t tile_bytes_n = (uint32_t)p.mma_n * 128u;   // bytes of one tap's weight rows
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int n_tile = p.m_major ? tile % p.n_tiles : tile / m_tiles, m = p.m_major ? tile / p.n_tiles : tile % m_tiles;
+      const int n_tile = p.m_major ? tile % p.n_tiles : tile / m_tiles, m = p.m_first + (p.m_major ? tile / p.n_tiles : tile % m_tiles);
       const int b = m / tiles_per_img, rem = m % tiles_per_img;
       const int oy0 = (rem / p.tiles_x) * TILE_H, ox0 = (rem % p.tiles_x) * item_w;
       const int n0 = n_tile * p.block_n;
@@ -441,7 +462,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
               float v0 = v[h][k][0] + bq.x + nz[h], v1 = v[h][k][1] + bq.y + nz[h];
               if (p.act == VT_ACT_LRELU) {
                 v0 = vt_lrelu(v0, sq.x) * p.gain; v1 = vt_lrelu(v1, sq.y) * p.gain;
-              } else if (p.act == VT_ACT_RELU_TANH) {
+              } else if (!WIDE && p.act == VT_ACT_RELU_TANH) {
                 v0 = tanhf(fmaxf(v0, 0.f)); v1 = tanhf(fmaxf(v1, 0.f));
               }
               const int64_t off = p.phase_off[ph] + off0[h] + ch;
@@ -454,7 +475,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
                 v0 *= p.alpha; v1 *= p.alpha;
               }
               if (p.round_tf32) { v0 = vt_round_tf32(v0); v1 = vt_round_tf32(v1); }
-              if (p.rgb_w) {
+              if (!WIDE && p.rgb_w) {
                 // 1x1 modulated conv to 3 channels on the values just produced (model/stylegan/model.py:384-385)
                 const float* w0 = p.rgb_w + ((int64_t)(p.wB > 1 ? b : 0) * 3) * p.Cout + ch;
 #pragma unroll
@@ -487,7 +508,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
               }
           }
         }
-        if (p.rgb_w) {
+        if (!WIDE && p.rgb_w) {
 #pragma unroll
           for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -506,8 +527,8 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
   }
 }
 
-// The instantiations conv_tc_run can select: every (MMA N, M tiles) with MT * NW <= MAX_ACC_COLS in each operand mode, and the
-// N-stacked form only at N = 64 (Cout == 32).
+// The instantiations conv_tc_run can select: every (MMA N, M tiles) with MT * NW <= MAX_ACC_COLS in each operand mode, the
+// N-stacked form only at N = 64 (Cout == 32), and the wide item (N = 256, one M tile) in the bf16 split mode.
 struct TcKernel {
   int nw, mt, op;
   void (*fn)(TcArgs);
@@ -517,6 +538,7 @@ struct TcKernel {
 const TcKernel kTcKernels[] = {
     VT_TC_OPS(128, 1), VT_TC_OPS(64, 1), VT_TC_OPS(64, 2), VT_TC_OPS(32, 1), VT_TC_OPS(32, 2), VT_TC_OPS(32, 4),
     {64, 1, OP_BF16_NSTACK, conv_tc_kernel<64, 1, OP_BF16_NSTACK>}, {64, 2, OP_BF16_NSTACK, conv_tc_kernel<64, 2, OP_BF16_NSTACK>},
+    {WIDE_N, 1, OP_BF16, conv_tc_kernel<WIDE_N, 1, OP_BF16>},
 };
 #undef VT_TC_OPS
 
@@ -572,6 +594,7 @@ int g_tc_s2_halo = 0;  // 1: stride-2 layers may use halo staging (4 parity-view
 int g_tc_stage_policy = 1;  // big halo boxes (dilated 3x3): 0 = shrink the weight ring first (3 + 3 stages at dilation 4), 1 = keep >= 5 weight stages and drop to 2 halo stages
 int g_tc_halo_pct = 60;    // halo staging must stage at most this percentage of the per-tap bytes (stride 1)
 int g_tc_m_major = 1;      // work items ordered pixel-tile-major (the N tiles of a pixel tile run side by side: the activations' second read hits L2)
+int g_tc_wide = 1;         // 128 x 256 work items: 0 = never, 1 = automatic (stride 1, with the wave-remainder split), 2 = whenever eligible, one launch
 
 int check_supported(const vt_conv_desc* d, bool set_err) {
 #define VT_SUP(cond, ...) do { if (!(cond)) { if (set_err) vt_set_error(__VA_ARGS__); return 0; } } while (0)
@@ -615,6 +638,7 @@ extern "C" int vt_set_option(const char* key, int value) {
   if (key && strcmp(key, "tc_halo_pct") == 0) { int old = g_tc_halo_pct; g_tc_halo_pct = value; return old; }
   if (key && strcmp(key, "tc_m_major") == 0) { int old = g_tc_m_major; g_tc_m_major = value; return old; }
   if (key && strcmp(key, "tc_transpose") == 0) { int old = g_tc_transpose; g_tc_transpose = value; return old; }
+  if (key && strcmp(key, "tc_wide") == 0) { int old = g_tc_wide; g_tc_wide = value; return old; }
   if (key && strcmp(key, "rs_kernel") == 0) { int old = g_rs_kernel; g_rs_kernel = value; return old; }
   if (key && strcmp(key, "instnorm_chunks") == 0) { int old = g_instnorm_chunks; g_instnorm_chunks = value; return old; }
   if (key && strcmp(key, "fir4") == 0) { int old = g_fir4; g_fir4 = value; return old; }
@@ -628,8 +652,9 @@ extern "C" int vt_conv2d_tc_supported(const vt_conv_desc* d) {
   return check_supported(d, false);
 }
 
-// chunks_out != NULL: plan only — how many instance-norm partial-sum chunks this descriptor's launch writes per (sample, channel)
-static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
+// chunks_out != NULL: plan only — how many instance-norm partial-sum chunks this descriptor's launch writes per (sample, channel).
+// m_first > 0: run only the pixel tiles from m_first on (the remainder launch of a wide layer); allow_wide = false: 128-wide N tiles.
+static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out, int m_first = 0, bool allow_wide = true) {
   if (vt_validate_conv_desc(d, "conv2d_tc")) return 1;
   if (!check_supported(d, true)) return 1;
 
@@ -698,12 +723,17 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
     dymin = vy < dymin ? vy : dymin; dymax = vy > dymax ? vy : dymax;
   }
 
-  // ---- N tile and accumulator plan (registers: mt * N <= 256 accumulator columns per consumer thread)
-  // GEMM N = n_phase * Cout (phase-major rows of the weight tensor); N tile = largest power of two <= 128 dividing it
+  // ---- N tile and accumulator plan (registers: mt * N <= 128 accumulator columns per consumer thread, or the wide item)
+  // GEMM N = n_phase * Cout (phase-major rows of the weight tensor); N tile = largest power of two <= 128 dividing it, or 256
+  // (the wide item) in the bf16 split mode when it divides N and its pipeline fits (below)
   const int n_eff = d->n_phase * d->Cout;
-  int bn = MAX_BLOCK_N;
-  while (bn > 32 && (n_eff % bn) != 0) bn /= 2;
-  VT_CHECK(n_eff % bn == 0, "conv_tc: no N tile for N=%d", n_eff);
+  int bn_narrow = MAX_BLOCK_N;
+  while (bn_narrow > 32 && (n_eff % bn_narrow) != 0) bn_narrow /= 2;
+  VT_CHECK(n_eff % bn_narrow == 0, "conv_tc: no N tile for N=%d", n_eff);
+  // (automatic: stride 1 only; the stride-2 layers, which stage one box per tap, measured slower with wide items)
+  const bool wide = allow_wide && (g_tc_wide == 2 || (g_tc_wide == 1 && d->stride == 1)) && op == OP_BF16 && n_eff % WIDE_N == 0 &&
+                    !d->rgb_w && d->act != VT_ACT_RELU_TANH;
+  const int bn = wide ? WIDE_N : bn_narrow;
   const int bnm = nstack ? 2 * bn : bn;  // MMA N = accumulator columns = weight rows per tile
   // halo staging: multi-tap layers (one box serves all taps) and small-N 1x1 layers (several M tiles per box and weight tile).
   // tc_mode 3: halo for stride 1 only (A/B tests)
@@ -784,6 +814,8 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
     smem_bytes = a.a_stages * a.a_stage_bytes + a.b_stages * a.b_stage_bytes + fixed;
     if (smem_bytes <= MAX_SMEM || mt == 1) break;
   }
+  // the wide item needs at least 2 A stages and 3 weight stages (32 KB each); otherwise the layer takes the 128-wide plan
+  if (wide && !(smem_bytes <= MAX_SMEM && a.a_stages >= 2 && a.b_stages >= 3)) return conv_tc_run(d, stream, chunks_out, m_first, false);
   a.b_tx_bytes = bnm * 128 * tgroup;
   VT_CHECK(smem_bytes <= MAX_SMEM && a.a_stages >= 2 && a.b_stages >= 2 && a.a_stages <= 8 && a.b_stages <= 8,
            "conv_tc: shared memory plan does not fit (%d B, mt=%d, bn=%d)", smem_bytes, mt, bn);
@@ -800,9 +832,12 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
   VT_CHECK(!d->rgb_w || a.n_tiles == 1, "conv_tc: fused ToRGB needs one N tile (Cout = %d)", d->Cout);
   a.tiles_x = (int)vt_cdiv(gWo, TILE_W * mt);
   a.tiles_y = (int)vt_cdiv(gHo, TILE_H);
-  const int64_t total = (int64_t)a.n_tiles * a.B * a.tiles_x * a.tiles_y;
+  const int64_t m_total = (int64_t)a.B * a.tiles_x * a.tiles_y;
+  VT_CHECK(m_first < m_total, "conv_tc: first pixel tile %d out of range", m_first);
+  const int64_t total = (int64_t)a.n_tiles * (m_total - m_first);
   VT_CHECK(total < (1LL << 31), "conv_tc: too many tiles");
   a.total_tiles = (int)total;
+  a.m_first = m_first;
   a.m_major = g_tc_m_major ? 1 : 0;
   {
     // fused instance-norm statistics of the output: one chunk per (pixel tile of an image, consumer warp)
@@ -876,10 +911,17 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out) {
     if (k.nw == bnm && k.mt == mt && k.op == op) kern = &k;
   if (!kern) return vt_set_error("conv_tc: no kernel for MMA N = %d, %d M tiles, operand mode %d", bnm, mt, op);
   int grid = vt_num_sms();
+  // Wave remainder of a wide layer: its whole rounds of wide items (one per SM) run in this launch, the pixel tiles left over
+  // in a second launch of 128-wide items, which fills the last partial round with half-length items.  Both use the same
+  // tiling and statistics chunks and write disjoint outputs.
+  int m_split = 0;
+  if (wide && g_tc_wide == 1 && a.total_tiles >= grid && a.total_tiles % grid != 0)
+    m_split = (a.total_tiles / grid) * grid / a.n_tiles;
+  if (m_split > 0) a.total_tiles = m_split * a.n_tiles;
   if (grid > a.total_tiles) grid = a.total_tiles;
   kern->fn<<<grid, TC_THREADS, smem_bytes, (cudaStream_t)stream>>>(a);
   VT_LAUNCH_CHECK();
-  return 0;
+  return m_split > 0 ? conv_tc_run(d, stream, nullptr, m_split, false) : 0;
 }
 
 extern "C" int vt_conv2d_tc_tf32(const vt_conv_desc* d, void* stream) { return conv_tc_run(d, stream, nullptr); }

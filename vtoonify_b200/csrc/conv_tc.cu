@@ -13,6 +13,8 @@
 //                                   kept in flight while the next stage is awaited; then the epilogue straight from the
 //                                   accumulator registers (+noise, +bias, leaky-relu*gain, residual, TF32 rna, fused ToRGB,
 //                                   instance-norm partial sums) with direct global stores.
+//                                   conv_tc_pingpong_kernel: each warpgroup owns alternate work items whole (all 128 pixels),
+//                                   so one item's epilogue runs under the other warpgroup's MMAs.
 //
 // A-operand reuse ("halo" mode, stride-1 convs): one TMA box of (8+2d) x (16+2d) pixels per 32-channel chunk serves all
 // 9 taps; each tap's MMA reads it through a descriptor whose start address is shifted by whole 128-byte rows and whose
@@ -46,7 +48,8 @@ constexpr int MAX_ACC_COLS = 128;             // accumulator columns per consume
                                               // budget of 168 registers per thread; 256 columns spill there
 // The wide work item: 128 pixels x 256 output channels on m64n256k16 (bf16 split only, one M tile).  Its 256 accumulator
 // columns (128 registers) fit because warpgroup 0 (producer + transform warps) hands registers to the two consumer
-// warpgroups with setmaxnreg: 128 * WIDE_REGS_XFORM + 256 * WIDE_REGS_CONSUMER <= 384 * 168, the launch allocation.
+// warpgroups with setmaxnreg: 128 * WIDE_REGS_XFORM + 256 * WIDE_REGS_CONSUMER <= 384 * 168, the launch allocation.  The
+// ping-pong item (two 64 x 128 accumulators per consumer thread) uses the same plan.
 constexpr int WIDE_N = 256;
 constexpr int WIDE_REGS_XFORM = 88;
 constexpr int WIDE_REGS_CONSUMER = 208;
@@ -155,17 +158,23 @@ __device__ __forceinline__ void mma_step(float* acc, uint64_t adesc, uint64_t bd
   }
 }
 
-// NW: MMA N (accumulator columns per M tile); MT: M tiles (accumulators) per work item; OP: operand mode (TcOp)
-template <int NW, int MT, int OP>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-conv_tc_kernel(const __grid_constant__ TcArgs p) {
-  // The wide item is the one instantiation that reallocates registers between the warpgroups.  Its epilogue leaves out the
-  // fused ToRGB and the tanh activation (the planner never gives it those layers): with them, the fully unrolled 8-chunk
-  // epilogue made the kernel 11.6k instructions, which no longer stay in the instruction cache, and every layer ran slower
-  // wide than 128-wide; without them it is 7.0k, the size of the 128-wide kernel.
+// NW: MMA N (accumulator columns per M tile); MT: M tiles (accumulators) per work item; OP: operand mode (TcOp);
+// PP: ping-pong (conv_tc_pingpong_kernel): each consumer warpgroup owns whole work items, both 64-row halves of every M tile
+template <int NW, int MT, int OP, bool PP>
+__device__ __forceinline__ void conv_tc_body(const TcArgs& p) {
+  // The wide item and the ping-pong item hold 128 accumulator registers per consumer thread; they are the instantiations that
+  // reallocate registers between the warpgroups.  Their epilogue leaves out the fused ToRGB and the tanh activation (the
+  // planner never gives them those layers): with them, the fully unrolled 8-chunk epilogue made the wide kernel 11.6k
+  // instructions, which no longer stay in the instruction cache, and every layer ran slower wide than 128-wide; without them
+  // it is 7.0k, the size of the 128-wide kernel.
   constexpr bool WIDE = NW == WIDE_N;
+  constexpr bool REALLOC = WIDE || PP;
+  constexpr int HALVES = PP ? 2 : 1;   // 64-row halves of an M tile one consumer warpgroup computes
   static_assert((MT * NW <= MAX_ACC_COLS || (WIDE && MT == 1 && OP == OP_BF16)) && (MT == 1 || MT == 2 || MT == 4),
                 "accumulators of one work item exceed the register plan");
+  static_assert(!PP || (NW == MAX_BLOCK_N && MT == 1 && OP == OP_BF16), "the ping-pong item is the 128 x 128 bf16-split item");
+  // ping-pong: a stage is released by the 4 warps of the warpgroup that owns the item reading it
+  constexpr int RELEASES = PP ? 4 : RELEASE_ARRIVALS;
   static_assert(128 * WIDE_REGS_XFORM + 256 * WIDE_REGS_CONSUMER <= TC_THREADS * ((65536 / TC_THREADS) & ~7),
                 "setmaxnreg plan exceeds the launch allocation");
   static_assert(OP != OP_BF16_NSTACK || NW == 64, "the N-stacked form is the Cout == 32 layer at MMA N = 64");
@@ -182,6 +191,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
   auto b_full = [&](int i) { return bar_base + 128u + 8u * i; };
   auto b_empty = [&](int i) { return bar_base + 192u + 8u * i; };
   auto a_ready = [&](int i) { return bar_base + 256u + 8u * i; };   // bf16x3: A stage converted to [hi|lo] 16-bit rows
+  auto turn = [&](int c) { return bar_base + 320u + 8u * c; };      // ping-pong: consumer warpgroup c may run its main loop
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
@@ -192,8 +202,9 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
     tma_prefetch_desc(&p.w_map);
   }
   if (warp == 1 && lane == 0) {
-    for (int i = 0; i < p.a_stages; ++i) { mbar_init(a_full(i), 1); mbar_init(a_empty(i), RELEASE_ARRIVALS); mbar_init(a_ready(i), XFORM_WARPS); }
-    for (int i = 0; i < p.b_stages; ++i) { mbar_init(b_full(i), 1); mbar_init(b_empty(i), RELEASE_ARRIVALS); }
+    for (int i = 0; i < p.a_stages; ++i) { mbar_init(a_full(i), 1); mbar_init(a_empty(i), RELEASES); mbar_init(a_ready(i), XFORM_WARPS); }
+    for (int i = 0; i < p.b_stages; ++i) { mbar_init(b_full(i), 1); mbar_init(b_empty(i), RELEASES); }
+    if constexpr (PP) { mbar_init(turn(0), 4); mbar_init(turn(1), 4); }
     fence_barrier_init();
     fence_proxy_async_smem();
   }
@@ -204,7 +215,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
   constexpr int item_w = TILE_W * MT;   // a work item covers item_w x TILE_H output pixels
 
   if (wg == 0) {
-    if constexpr (WIDE) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WIDE_REGS_XFORM));
+    if constexpr (REALLOC) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WIDE_REGS_XFORM));
     if (warp == 0) {
       // ================= TMA producer (whole warp converged; one elected lane issues) =================
       int a_st = 0, b_st = 0;
@@ -342,25 +353,75 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
     }
   } else {
     // ================= consumers: wgmma main loop + epilogue =================
-    if constexpr (WIDE) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WIDE_REGS_CONSUMER));
-    const int c = wg - 1;                       // pixel rows [8c, 8c + 8) of the 8 x 16 tile
+    // Cooperative (PP = false): both warpgroups work on every item, warpgroup c on pixel rows [8c, 8c + 8) of the 8 x 16 tile,
+    // and every stage is released by all 8 consumer warps.
+    // Ping-pong (PP = true): warpgroup c owns the CTA's items k with k % 2 == c and computes all 16 rows of them, so its
+    // epilogue runs while the other warpgroup's MMAs keep the tensor cores busy.  Invariants:
+    //   * the producer and the transform warps fill the stages in the cooperative order; a stage use is released once, by the
+    //     4 warps of the warpgroup whose item reads it (empty barriers count 4);
+    //   * the warpgroup that does not own item k reads none of its stages and does not wait for them: it only advances its
+    //     ring indices and parities over them, by the stage counts the plan fixes per item (a_item halo or per-tap stages,
+    //     b_item weight stages);
+    //   * the main loops run in item order: warpgroup c waits on turn(c) before item k's first stage (k > 0) and arrives on
+    //     turn(1 - c) after item k's last commit.  So every stage use before item k has been waited on (its full phase has
+    //     completed) when item k's owner waits for its own phase: an mbarrier parity wait never sees a phase two steps away;
+    //   * a CTA whose item count is odd, or 1, just leaves the last hand-off unwaited.
+    if constexpr (REALLOC) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WIDE_REGS_CONSUMER));
+    const int c = wg - 1;
     const int tw_ = (threadIdx.x & 127) >> 5;   // warp inside the warpgroup: accumulator rows [16 tw_, 16 tw_ + 16)
     const bool leader = lane == 0;   // one arrival per consumer warp
     const int qd = lane & 3;                    // column pair inside each 8-column group
-    float acc[MT][NW / 2];
+    float acc[MT * HALVES][NW / 2];
 #pragma unroll
-    for (int g = 0; g < MT; ++g)
+    for (int g = 0; g < MT * HALVES; ++g)
 #pragma unroll
       for (int i = 0; i < NW / 2; ++i) acc[g][i] = 0.f;
     const float nw = (p.noise && p.noise_w) ? *p.noise_w : 0.f;
     int a_st = 0, b_st = 0;
     uint32_t a_par = 0, b_par = 0;
     const uint32_t tile_bytes_n = (uint32_t)p.mma_n * 128u;   // bytes of one tap's weight rows
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    int a_item = 0, b_item = 0;   // ping-pong: A and weight stages of one work item
+    uint32_t t_par = 0;
+    if constexpr (PP) {
+      for (int s = 0; s < p.n_src; ++s) {
+        a_item += p.halo ? p.kchunks[s] : p.kchunks[s] * p.n_steps;
+        b_item += p.kchunks[s] * (p.n_steps / p.tgroup);
+      }
+    }
+    for (int tile = blockIdx.x, item = 0; tile < p.total_tiles; tile += gridDim.x, ++item) {
       const int n_tile = p.m_major ? tile % p.n_tiles : tile / m_tiles, m = p.m_first + (p.m_major ? tile / p.n_tiles : tile % m_tiles);
       const int b = m / tiles_per_img, rem = m % tiles_per_img;
       const int oy0 = (rem / p.tiles_x) * TILE_H, ox0 = (rem % p.tiles_x) * item_w;
       const int n0 = n_tile * p.block_n;
+      if constexpr (PP) {
+        if ((item & 1) != c) {
+          for (a_st += a_item; a_st >= p.a_stages; a_st -= p.a_stages) a_par ^= 1;
+          for (b_st += b_item; b_st >= p.b_stages; b_st -= p.b_stages) b_par ^= 1;
+          continue;
+        }
+        // The epilogue's global reads are requested now and land while the MMAs run: the noise of every pixel this thread
+        // stores (each phase of a folded up-convolution is its own word) into L1, and the thread's 128-byte line of each
+        // pixel's residual row into L2 (an item's residual is 64 KB, more than the L1 left beside the pipeline's shared memory).
+        const int ph_first = n0 / p.Cout, ph_last = (n0 + p.block_n - 1) / p.Cout;
+#pragma unroll
+        for (int hh = 0; hh < HALVES; ++hh)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = 64 * hh + 16 * tw_ + (lane >> 2);
+            const int oy = oy0 + r / TILE_W + h, ox = ox0 + r % TILE_W;
+            if (oy >= p.Ho || ox >= p.Wo) continue;
+            if (p.noise) {
+              const int64_t pix = (int64_t)b * p.pix_sb + (int64_t)oy * p.pix_sy + (int64_t)ox * p.pix_sx;
+              for (int ph = ph_first; ph <= ph_last; ++ph) asm volatile("prefetch.global.L1 [%0];" ::"l"(p.noise + p.phase_pix[ph] + pix));
+            }
+            if (p.res) {
+              const int64_t off = p.phase_off[ph_first] + (int64_t)b * p.out_sb + (int64_t)oy * p.out_sy + (int64_t)ox * p.out_sx +
+                                  (n0 - ph_first * p.Cout) + 32 * qd;
+              asm volatile("prefetch.global.L2 [%0];" ::"l"(p.res + off));
+            }
+          }
+        if (item > 0) { mbar_wait(turn(c), t_par); t_par ^= 1; }
+      }
       uint32_t first = 1;   // first K step of this work item overwrites the accumulators
       int rel_a = -1, rel_b = -1;   // stages the previous (still in flight) wgmma group reads, released once it has completed
       for (int s = 0; s < p.n_src; ++s) {
@@ -378,15 +439,17 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
               a_addr += (uint32_t)p.step_aoff[j];
               sbo = (uint32_t)p.step_sbo[j];
             }
-            a_addr += 8u * (uint32_t)c * sbo;   // this warpgroup's 8 pixel rows = 8 row groups of 8 pixels
+            if constexpr (!PP) a_addr += 8u * (uint32_t)c * sbo;   // this warpgroup's 8 pixel rows = 8 row groups of 8 pixels
             const uint64_t bdesc = make_smem_desc_sw128(b_base + b_st * p.b_stage_bytes + (uint32_t)gj * tile_bytes_n, 1024);
             const bool last_of_group = (gj == p.tgroup - 1);
             wgmma_fence();
 #pragma unroll
-            for (int g = 0; g < MT; ++g) {
-              const uint64_t adesc = make_smem_desc_sw128(a_addr + (uint32_t)(g * TILE_W * 128), sbo);
-              mma_step<NW, OP>(acc[g], adesc, bdesc, first);
-            }
+            for (int g = 0; g < MT; ++g)
+#pragma unroll
+              for (int hh = 0; hh < HALVES; ++hh) {
+                const uint64_t adesc = make_smem_desc_sw128(a_addr + 8u * (uint32_t)hh * sbo + (uint32_t)(g * TILE_W * 128), sbo);
+                mma_step<NW, OP>(acc[g * HALVES + hh], adesc, bdesc, first);
+              }
             wgmma_commit();
             wgmma_wait<1>();   // this warp's share of the group before this one has completed: its stages may be refilled
             if (leader) {
@@ -401,9 +464,12 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
           }
         }
       }
+      if constexpr (PP) {
+        if (leader) mbar_arrive(turn(c ^ 1));   // every stage of this item has been waited on: the other warpgroup's item may start
+      }
       wgmma_wait<0>();
 #pragma unroll
-      for (int g = 0; g < MT; ++g) wgmma_pin<NW / 2>(acc[g]);
+      for (int g = 0; g < MT * HALVES; ++g) wgmma_pin<NW / 2>(acc[g]);
       if (leader) {
         if (rel_a >= 0) mbar_arrive(a_empty(rel_a));
         if (rel_b >= 0) mbar_arrive(b_empty(rel_b));
@@ -411,12 +477,14 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
 
       // ---- epilogue. Accumulator register i of a thread holds row 16 tw_ + lane/4 + 8 ((i/2)%2) (a pixel of the tile) and
       // column 8 (i/4) + 2 qd + (i%2): every thread owns two pixels (same x, rows ty and ty + 1) and 2-channel pairs of them.
-      const int r0 = 64 * c + 16 * tw_ + (lane >> 2);
-      const int ty = r0 / TILE_W, tx = r0 % TILE_W;   // second pixel: ty + 1
+      // Half hh (ping-pong) or warpgroup c (cooperative) selects pixel rows [8 hh, 8 hh + 8) of the tile.
       const int ph0 = n0 / p.Cout, nb0 = n0 - ph0 * p.Cout;
       const int nchunks = p.block_n / 32;
 #pragma unroll
-      for (int g = 0; g < MT; ++g) {
+      for (int gh = 0; gh < MT * HALVES; ++gh) {
+        const int g = gh / HALVES, half = PP ? gh % HALVES : c;
+        const int r0 = 64 * half + 16 * tw_ + (lane >> 2);
+        const int ty = r0 / TILE_W, tx = r0 % TILE_W;   // second pixel: ty + 1
         int oy[2], ox[2];
         bool in_img[2];
         int64_t off0[2], pix0[2];
@@ -447,8 +515,8 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const int i = 16 * j + 4 * k + 2 * h + e;
-                float x = acc[g][i];
-                if constexpr (OP == OP_BF16_NSTACK) x += acc[g][(i + 16) % (NW / 2)];   // second column half: the w_lo products
+                float x = acc[gh][i];
+                if constexpr (OP == OP_BF16_NSTACK) x += acc[gh][(i + 16) % (NW / 2)];   // second column half: the w_lo products
                 v[h][k][e] = x * p.acc_scale;
               }
 #pragma unroll
@@ -462,7 +530,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
               float v0 = v[h][k][0] + bq.x + nz[h], v1 = v[h][k][1] + bq.y + nz[h];
               if (p.act == VT_ACT_LRELU) {
                 v0 = vt_lrelu(v0, sq.x) * p.gain; v1 = vt_lrelu(v1, sq.y) * p.gain;
-              } else if (!WIDE && p.act == VT_ACT_RELU_TANH) {
+              } else if (!REALLOC && p.act == VT_ACT_RELU_TANH) {
                 v0 = tanhf(fmaxf(v0, 0.f)); v1 = tanhf(fmaxf(v1, 0.f));
               }
               const int64_t off = p.phase_off[ph] + off0[h] + ch;
@@ -475,7 +543,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
                 v0 *= p.alpha; v1 *= p.alpha;
               }
               if (p.round_tf32) { v0 = vt_round_tf32(v0); v1 = vt_round_tf32(v1); }
-              if (!WIDE && p.rgb_w) {
+              if (!REALLOC && p.rgb_w) {
                 // 1x1 modulated conv to 3 channels on the values just produced (model/stylegan/model.py:384-385)
                 const float* w0 = p.rgb_w + ((int64_t)(p.wB > 1 ? b : 0) * 3) * p.Cout + ch;
 #pragma unroll
@@ -491,7 +559,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
           if (p.stats_ws) {
             // AdaptiveInstanceNorm statistics of the tensor this launch writes (model/dualstylegan.py:10-21): per channel, the
             // warp's 16 pixels summed in a fixed butterfly order (no atomics), pixels outside the image masked
-            const int kchunk = ((rem * MT + g) * STATS_WARPS) + c * 4 + tw_;
+            const int kchunk = ((rem * MT + g) * STATS_WARPS) + half * 4 + tw_;
             float2* wsp = reinterpret_cast<float2*>(p.stats_ws) + ((int64_t)kchunk * p.B + b) * p.Cout + nb + 2 * qd;
 #pragma unroll
             for (int k = 0; k < 4; ++k)
@@ -508,7 +576,7 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
               }
           }
         }
-        if (!WIDE && p.rgb_w) {
+        if (!REALLOC && p.rgb_w) {
 #pragma unroll
           for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -527,18 +595,31 @@ conv_tc_kernel(const __grid_constant__ TcArgs p) {
   }
 }
 
+template <int NW, int MT, int OP>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+conv_tc_kernel(const __grid_constant__ TcArgs p) { conv_tc_body<NW, MT, OP, false>(p); }
+
+// The ping-pong form has its own name: it is the other instantiation besides the wide item whose warpgroups reallocate
+// registers, and profiles tell the two schedules apart.
+template <int NW, int MT, int OP>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+conv_tc_pingpong_kernel(const __grid_constant__ TcArgs p) { conv_tc_body<NW, MT, OP, true>(p); }
+
 // The instantiations conv_tc_run can select: every (MMA N, M tiles) with MT * NW <= MAX_ACC_COLS in each operand mode, the
-// N-stacked form only at N = 64 (Cout == 32), and the wide item (N = 256, one M tile) in the bf16 split mode.
+// N-stacked form only at N = 64 (Cout == 32), the wide item (N = 256, one M tile) in the bf16 split mode, and the ping-pong
+// form of the 128 x 128 bf16-split item.
 struct TcKernel {
   int nw, mt, op;
+  bool pp;
   void (*fn)(TcArgs);
 };
-#define VT_TC_OPS(NW, MT) {NW, MT, OP_TF32, conv_tc_kernel<NW, MT, OP_TF32>}, {NW, MT, OP_BF16, conv_tc_kernel<NW, MT, OP_BF16>}, \
-                          {NW, MT, OP_F16, conv_tc_kernel<NW, MT, OP_F16>}
+#define VT_TC_OPS(NW, MT) {NW, MT, OP_TF32, false, conv_tc_kernel<NW, MT, OP_TF32>}, {NW, MT, OP_BF16, false, conv_tc_kernel<NW, MT, OP_BF16>}, \
+                          {NW, MT, OP_F16, false, conv_tc_kernel<NW, MT, OP_F16>}
 const TcKernel kTcKernels[] = {
     VT_TC_OPS(128, 1), VT_TC_OPS(64, 1), VT_TC_OPS(64, 2), VT_TC_OPS(32, 1), VT_TC_OPS(32, 2), VT_TC_OPS(32, 4),
-    {64, 1, OP_BF16_NSTACK, conv_tc_kernel<64, 1, OP_BF16_NSTACK>}, {64, 2, OP_BF16_NSTACK, conv_tc_kernel<64, 2, OP_BF16_NSTACK>},
-    {WIDE_N, 1, OP_BF16, conv_tc_kernel<WIDE_N, 1, OP_BF16>},
+    {64, 1, OP_BF16_NSTACK, false, conv_tc_kernel<64, 1, OP_BF16_NSTACK>}, {64, 2, OP_BF16_NSTACK, false, conv_tc_kernel<64, 2, OP_BF16_NSTACK>},
+    {WIDE_N, 1, OP_BF16, false, conv_tc_kernel<WIDE_N, 1, OP_BF16>},
+    {MAX_BLOCK_N, 1, OP_BF16, true, conv_tc_pingpong_kernel<MAX_BLOCK_N, 1, OP_BF16>},
 };
 #undef VT_TC_OPS
 
@@ -595,6 +676,7 @@ int g_tc_stage_policy = 1;  // big halo boxes (dilated 3x3): 0 = shrink the weig
 int g_tc_halo_pct = 60;    // halo staging must stage at most this percentage of the per-tap bytes (stride 1)
 int g_tc_m_major = 1;      // work items ordered pixel-tile-major (the N tiles of a pixel tile run side by side: the activations' second read hits L2)
 int g_tc_wide = 1;         // 128 x 256 work items: 0 = never, 1 = automatic (stride 1, with the wave-remainder split), 2 = whenever eligible, one launch
+int g_tc_pingpong = 1;     // 128 x 128 bf16-split items owned by one consumer warpgroup each: 0 = never, 1 = automatic (>= 3 items per CTA), 2 = whenever eligible
 
 int check_supported(const vt_conv_desc* d, bool set_err) {
 #define VT_SUP(cond, ...) do { if (!(cond)) { if (set_err) vt_set_error(__VA_ARGS__); return 0; } } while (0)
@@ -639,6 +721,7 @@ extern "C" int vt_set_option(const char* key, int value) {
   if (key && strcmp(key, "tc_m_major") == 0) { int old = g_tc_m_major; g_tc_m_major = value; return old; }
   if (key && strcmp(key, "tc_transpose") == 0) { int old = g_tc_transpose; g_tc_transpose = value; return old; }
   if (key && strcmp(key, "tc_wide") == 0) { int old = g_tc_wide; g_tc_wide = value; return old; }
+  if (key && strcmp(key, "tc_pingpong") == 0) { int old = g_tc_pingpong; g_tc_pingpong = value; return old; }
   if (key && strcmp(key, "rs_kernel") == 0) { int old = g_rs_kernel; g_rs_kernel = value; return old; }
   if (key && strcmp(key, "instnorm_chunks") == 0) { int old = g_instnorm_chunks; g_instnorm_chunks = value; return old; }
   if (key && strcmp(key, "fir4") == 0) { int old = g_fir4; g_fir4 = value; return old; }
@@ -906,9 +989,14 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out, int
       if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
   });
   VT_CHECK(attr_err == cudaSuccess, "conv_tc: cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err));
+  // ping-pong: never with the fused ToRGB or tanh, which it leaves out.  Automatic: when every CTA gets at least 3 items.  Ping-pong
+  // hides the epilogues of all but the last item of a CTA, but one warpgroup alone runs an item's main loop slower than two: one
+  // item per CTA measured 3-9 % slower, two gave no clear gain, three or more 2-21 % faster (DESIGN.md section 4).
+  const bool pingpong = (g_tc_pingpong == 2 || (g_tc_pingpong == 1 && a.total_tiles >= 3 * vt_num_sms())) && op == OP_BF16 &&
+                        bnm == MAX_BLOCK_N && mt == 1 && !d->rgb_w && d->act != VT_ACT_RELU_TANH;
   const TcKernel* kern = nullptr;
   for (const TcKernel& k : kTcKernels)
-    if (k.nw == bnm && k.mt == mt && k.op == op) kern = &k;
+    if (k.nw == bnm && k.mt == mt && k.op == op && k.pp == pingpong) kern = &k;
   if (!kern) return vt_set_error("conv_tc: no kernel for MMA N = %d, %d M tiles, operand mode %d", bnm, mt, op);
   int grid = vt_num_sms();
   // Wave remainder of a wide layer: its whole rounds of wide items (one per SM) run in this launch, the pixel tiles left over

@@ -86,8 +86,9 @@ class AdaResBlock(nn.Module):
 
 
 class DualStyleGAN(ops.WeightsEpochMixin, nn.Module):
-    """model/dualstylegan.py:47-76 constructor (parameters / keys); VToonify only uses ``.style``, ``.res[7:]``
-    and ``.generator`` at inference (model/vtoonify.py:214-224, 279-283)."""
+    """model/dualstylegan.py:47-203: same constructor, parameters / keys and ``forward`` keyword interface (forward only).
+    VToonify uses ``.style``, ``.res[7:]`` and ``.generator`` (model/vtoonify.py:214-224, 279-283); ``forward`` is the
+    exemplar-based synthesis with the extrinsic style path, the frozen teacher of VToonify-D training."""
 
     def __init__(self, size, style_dim, n_mlp, channel_multiplier=2, twoRes=True, res_index=6):
         super().__init__()
@@ -116,3 +117,82 @@ class DualStyleGAN(ops.WeightsEpochMixin, nn.Module):
         self.num_layers = self.generator.num_layers
         self.n_latent = self.generator.n_latent
         self.channels = self.generator.channels
+
+    def forward(self, styles, exstyles, return_latents=False, return_feat=False, inject_index=None, truncation=1,
+                truncation_latent=None, input_is_latent=False, noise=None, randomize_noise=True, z_plus_latent=False,
+                use_res=True, fuse_index=18, interp_weights=[1] * 18):
+        """model/dualstylegan.py:84-194 -> ``(image, latent | None)``, or ``(feat, skip)`` with ``return_feat``."""
+        G = self.generator
+        latent, noise, cacheable = G._prepare(styles, inject_index, truncation, truncation_latent, input_is_latent, noise,
+                                              randomize_noise, z_plus_latent)
+        weights = tuple(float(w) for w in interp_weights)
+        token = None
+        if cacheable:
+            # every style-only tensor (extrinsic codes, blended styles, modulated weights, AdaIN rows) is memoised while the caller
+            # passes the same unmodified latent and exstyles objects with the same weights and path selection
+            ex_token = ops.style_token(self.style, exstyles)[0] if use_res else None
+            token = ops.style_token(self, latent, (ex_token, weights, fuse_index, bool(use_res)))[0]
+        with ops.style_scope(token):
+            feat, image = self._synthesis(latent, exstyles, noise, return_feat, use_res, fuse_index, weights)
+        if feat is not None:
+            return feat, image
+        return image, (latent if return_latents else None)
+
+    def _synthesis(self, latent, exstyles, noise, return_feat, use_res, fuse_index, w):
+        """model/dualstylegan.py:147-188 on NHWC activations -> ``(feat, skip image)``; ``feat`` (an NCHW view of the
+        activation) is None unless ``return_feat`` stopped the loop after the first level above ``res_index``."""
+        G = self.generator
+        if use_res:         # the colour transform T_c on the extrinsic code, for the ModRes blocks
+            resstyles = ops.style_cached(self, "resstyles",
+                                         lambda: self.style(exstyles.reshape(-1, exstyles.shape[-1])).reshape(exstyles.shape))
+
+        def per_layer(t, j):            # a [B, 512] code stands for every layer (the reference repeats it)
+            return t if t.ndim == 2 else t[:, j]
+
+        def modres(j):                  # a ModRes block follows conv layer j; weight 0 makes it the identity, so it is absent
+            return use_res and fuse_index >= max(j, 1) and j <= self.res_index and w[j] != 0
+
+        def style(j):                   # layer j's style: above res_index, the blend with the structure transform T_s
+            if not (use_res and fuse_index >= j and j > self.res_index) or w[j] == 0:
+                return latent[:, j]     # (weight 0: exactly the intrinsic code)
+            return ops.style_cached(self, f"style{j}", lambda: ops.axpby(self.res[j](per_layer(exstyles, j)), latent[:, j], w[j],
+                                                                          1.0 - w[j], round_tf32=False))
+
+        def styled(conv, x, j, n):      # StyledConv j and its ModRes block, which takes the conv's output statistics
+            if not modres(j):
+                return conv.forward_nhwc(x, style(j), noise=n)
+            st = None
+            if ops.affine_fusable():
+                x, st = conv.forward_nhwc(x, style(j), noise=n, want_stats=True)
+            else:
+                x = conv.forward_nhwc(x, style(j), noise=n)
+            return self.res[j].forward_nhwc(x, per_layer(resstyles, j), w[j], x_stats=st)
+
+        out = styled(G.conv1, ops.to_nhwc(G.input(latent)), 0, noise[0])
+        skip = G.to_rgb1.forward_nhwc(out, latent[:, 1])
+        i = 1
+        n_levels = len(G.to_rgbs)
+        for lvl, (conv1, conv2, noise1, noise2, to_rgb) in enumerate(zip(G.convs[::2], G.convs[1::2], noise[1::2], noise[2::2],
+                                                                         G.to_rgbs)):
+            out = styled(conv1, out, i, noise1)
+            feat_here = return_feat and i + 2 > self.res_index
+            if modres(i + 1):
+                # ToRGB reads the ModRes output: its own launch
+                out = styled(conv2, out, i + 1, noise2)
+                skip = to_rgb.forward_nhwc(out, style(i + 2), skip)
+            else:
+                out, skip = conv2.forward_nhwc(out, style(i + 1), noise=noise2, to_rgb=(to_rgb, style(i + 2), skip),
+                                               rgb_only=lvl == n_levels - 1 and not feat_here)
+            i += 2
+            if feat_here:
+                return ops.nhwc_as_nchw_view(out), skip
+        return None, skip
+
+    def make_noise(self):
+        return self.generator.make_noise()
+
+    def mean_latent(self, n_latent):
+        return self.generator.mean_latent(n_latent)
+
+    def get_latent(self, input):
+        return self.generator.style(input)

@@ -204,9 +204,14 @@ class ModulatedConv2d(nn.Module):
                                                             self.modulation.weight._version, self.modulation.bias._version))
 
     def forward_nhwc(self, x, style, externalweight=None, bias=None, noise=None, noise_w=None, act=False,
-                     slope=0.2, gain=ops.SQRT2, rgb=None):
+                     slope=0.2, gain=ops.SQRT2, rgb=None, want_stats=False):
         """x NHWC -> NHWC.  Optional fused StyledConv epilogue (noise, bias, leaky relu) and fused ToRGB tail
-        (``rgb`` dict, plain 3x3 form only: returns ``(out, rgb_image)``)."""
+        (``rgb`` dict, plain 3x3 form only: returns ``(out, rgb_image)``).  ``want_stats``: returns ``(out, instance-norm
+        statistics of out)``; the plain form takes them from the convolution's epilogue, the resampling forms from a separate
+        statistics pass."""
+        if want_stats and (self.upsample or self.downsample):
+            out = self.forward_nhwc(x, style, externalweight, bias, noise, noise_w, act, slope, gain)
+            return out, ops.instnorm_stats(out)
         B, H, W, Cs = x.shape
         k = self.kernel_size
         a = ACT_LRELU if act else ACT_NONE
@@ -232,7 +237,7 @@ class ModulatedConv2d(nn.Module):
             return ops.conv2d_nhwc([xb], w, ops.conv_taps(k, 0), 2, Ho, Wo, bias=bias, noise=noise, noise_w=noise_w,
                                    act=a, slope=slope, gain=gain)
         return ops.conv2d_nhwc([x], w, ops.conv_taps(k, self.padding), 1, H, W, bias=bias, noise=noise,
-                               noise_w=noise_w, act=a, slope=slope, gain=gain, rgb=rgb)
+                               noise_w=noise_w, act=a, slope=slope, gain=gain, rgb=rgb, want_stats=want_stats)
 
     def forward(self, input, style, externalweight=None):
         C = input.shape[1]
@@ -289,11 +294,13 @@ class StyledConv(nn.Module):
         self.noise = NoiseInjection()
         self.activate = FusedLeakyReLU(out_channel)
 
-    def forward_nhwc(self, x, style, noise=None, externalweight=None, zero_noise=False, to_rgb=None, rgb_only=False):
+    def forward_nhwc(self, x, style, noise=None, externalweight=None, zero_noise=False, to_rgb=None, rgb_only=False,
+                     want_stats=False):
         """``to_rgb`` = (ToRGB module, its style, skip image or None): also returns the RGB image, computed in this
         conv's epilogue when possible (the activation is then never re-read for the 1x1 ToRGB conv).  ``rgb_only``: the
         caller drops the activation (last layer of the synthesis network): the returned ``out`` may be ``None`` and a fused
-        launch does not write it to HBM at all."""
+        launch does not write it to HBM at all.  ``want_stats`` (without ``to_rgb``): returns ``(out, instance-norm
+        statistics of out)`` for an AdaIN consumer (ModulatedConv2d.forward_nhwc)."""
         B, H, W, _ = x.shape
         Ho, Wo = (2 * H, 2 * W) if self.conv.upsample else (H, W)
         if zero_noise:
@@ -305,7 +312,9 @@ class StyledConv(nn.Module):
         kw = dict(bias=self.activate.bias, noise=noise, noise_w=None if noise is None else self.noise.weight, act=True,
                   slope=self.activate.negative_slope, gain=self.activate.scale)
         if to_rgb is None:
-            return self.conv.forward_nhwc(x, style, externalweight, **kw)
+            return self.conv.forward_nhwc(x, style, externalweight, want_stats=want_stats, **kw)
+        if want_stats:
+            raise ValueError("StyledConv.forward_nhwc: want_stats and to_rgb are exclusive")
         trgb, style_rgb, skip = to_rgb
         Cout = self.conv.out_channel
         fuse = (ops.rgb_fusable(Cout) and not self.conv.upsample and not self.conv.downsample and trgb.fusable_skip(skip, H, W))
@@ -418,9 +427,11 @@ class Generator(ops.WeightsEpochMixin, nn.Module):
             return torch.cat([widen(styles[0], inject_index), widen(styles[1], self.n_latent - inject_index)], 1)
         return torch.cat([styles[0][:, :inject_index], styles[1][:, inject_index:]], 1)
 
-    def forward(self, styles, return_latents=False, inject_index=None, truncation=1, truncation_latent=None,
-                input_is_latent=False, noise=None, randomize_noise=True, z_plus_latent=False,
-                return_feature_ind=999):
+    def _prepare(self, styles, inject_index, truncation, truncation_latent, input_is_latent, noise, randomize_noise,
+                 z_plus_latent):
+        """Head of ``forward`` (model.py:517-565): mapping network, noise list, truncation, W+ code -> ``(latent, noise,
+        cacheable)``.  ``cacheable``: the latent is the caller's own tensor and nothing else shapes it (single style input
+        already in W+, no truncation / mixing), so per-latent caching keyed on that tensor object is valid."""
         if not input_is_latent:
             if not z_plus_latent:
                 styles = [self.style(s) for s in styles]
@@ -434,9 +445,15 @@ class Generator(ops.WeightsEpochMixin, nn.Module):
         if truncation < 1:
             styles = [truncation_latent + truncation * (s - truncation_latent) for s in styles]
         latent = self._latent(styles, inject_index)
-        # per-latent caching of the modulated weights: valid while the caller passes the same (unmodified) tensor object again
-        # and nothing else shapes the latent (single style input, no truncation / mixing)
         cacheable = len(styles) == 1 and input_is_latent and truncation >= 1 and latent is styles[0]
+        return latent, noise, cacheable
+
+    def forward(self, styles, return_latents=False, inject_index=None, truncation=1, truncation_latent=None,
+                input_is_latent=False, noise=None, randomize_noise=True, z_plus_latent=False,
+                return_feature_ind=999):
+        latent, noise, cacheable = self._prepare(styles, inject_index, truncation, truncation_latent, input_is_latent, noise,
+                                                 randomize_noise, z_plus_latent)
+        # per-latent caching of the modulated weights: valid while the caller passes the same (unmodified) tensor object again
         token = ops.style_token(self, latent)[0] if cacheable else None
         with ops.style_scope(token):
             return self._synthesis(latent, noise, return_latents, return_feature_ind)

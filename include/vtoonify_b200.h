@@ -36,13 +36,15 @@
 extern "C" {
 #endif
 
-#define VT_ABI_VERSION 6   /* 2: vt_conv_desc gained weight_bf16x3 / bf16x3_nstack / src_scale, vt_smalln_desc src_mask / tsum, vt_split_weights_bf16x3
+#define VT_ABI_VERSION 7   /* 2: vt_conv_desc gained weight_bf16x3 / bf16x3_nstack / src_scale, vt_smalln_desc src_mask / tsum, vt_split_weights_bf16x3
                             * 3: face-parsing helpers (vt_frame_s2d_f32 .. vt_logits_readout_f32 with out_bstride), backward ops, frame pre-filter
                             * 4: row-strip kernels, vt_conv_desc gained split_fmt / acc_scale
                             * 5: vt_conv_desc gained stats_ws / stats_ws_floats (statistics of the conv output), vt_conv2d_tc_stats_chunks,
                             *    vt_instnorm_finalize_f32
                             * 6: sm_90a: vt_conv2d_rs takes the vt_conv2d_tc_tf32 weight split; the row-strip up-conv, vt_set_debug_buffer and
-                            *    vt_selftest_tc_gemm are gone */
+                            *    vt_selftest_tc_gemm are gone
+                            * 7: instance-norm partials are pivoted: (pivot, sum and square sum of x - pivot) plus a per-chunk pixel
+                            *    count, sized by vt_instnorm_partials_floats */
 
 /* ---- library info / errors ------------------------------------------------------------- */
 int         vt_abi_version(void);
@@ -184,11 +186,12 @@ typedef struct vt_conv_desc {
                                  * 1 = fp16 hi + lo (vt_split_weights_f16x3: 11 + 11 mantissa bits, |activation| < 1.3e5)           */
   float   acc_scale;            /* accumulators are multiplied by this before the epilogue (0 = 1): the inverse of the power-of-two
                                  * `scale` given to vt_split_weights_f16x3                                                           */
-  float*  stats_ws;             /* optional (tensor-core kernel, n_phase == 1, no fused ToRGB): instance-norm partial sums of the tensor
-                                 * this launch WRITES, [chunks][B][Cout][2] = (sum, sum of squares) with chunks =
-                                 * vt_conv2d_tc_stats_chunks(desc); vt_instnorm_finalize_f32 turns them into (mean, rstd).  Replaces the
-                                 * separate statistics pass of AdaptiveInstanceNorm (model/dualstylegan.py:10-21) over a conv output   */
-  int64_t stats_ws_floats;      /* capacity of stats_ws in floats                                                                    */
+  float*  stats_ws;             /* optional (tensor-core kernel, n_phase == 1, no fused ToRGB): instance-norm partials of the tensor
+                                 * this launch WRITES, in the layout of vt_instnorm_finalize_f32 with chunks =
+                                 * vt_conv2d_tc_stats_chunks(desc) and Cs = Cout; vt_instnorm_finalize_f32 turns them into (mean, rstd).
+                                 * Replaces the separate statistics pass of AdaptiveInstanceNorm (model/dualstylegan.py:10-21) over a
+                                 * conv output                                                                                        */
+  int64_t stats_ws_floats;      /* capacity of stats_ws in floats: >= vt_instnorm_partials_floats(chunks, B, Cout)                   */
 } vt_conv_desc;
 
 /* fp32-exact CUDA-core implicit GEMM (FFMA). Any shape. */
@@ -292,13 +295,20 @@ int vt_fir_nhwc_f32(const float* in, const float* kernel, float* out, int B, int
 /* ---- a7: instance-norm statistics + AdaIN apply (NHWC) ------------------------------------ */
 /* mode 0: x = in[b,p,c] (c < C). mode 1: virtual cat(in, |in - in2|) with 2C channels.
  * stats: [B, Cs, 2] = (mean, rstd) with biased variance, eps inside rsqrt.  Deterministic two-stage reduction (no
- * atomics); ws: caller-allocated scratch of vt_instnorm_ws_bytes() bytes. */
+ * atomics): centred per-chunk partials, then vt_instnorm_finalize_f32; ws: caller-allocated scratch of vt_instnorm_ws_bytes() bytes. */
 int64_t vt_instnorm_ws_bytes(int B, int64_t HW, int C, int mode);
 int vt_instnorm_stats_nhwc(const float* in, const float* in2, int mode, int B, int64_t HW, int C, int c_stride,
                            float eps, float* stats, void* ws, void* stream);
-/* second stage alone: partial sums ws [chunks][B*Cs][2] = (sum, sum of squares) over HW pixels per entry -> stats [B, Cs, 2] = (mean, rstd);
- * chunks are added in index order in double precision.  Used with vt_conv_desc.stats_ws (partial sums written by the producing conv). */
+/* second stage alone.  ws holds three float arrays of E = chunks * B * Cs entries (entry chunk * B * Cs + b * Cs + c): a pivot k
+ * near the chunk's values (a value of the chunk, or its rounded mean), the sum of (x - k) and the sum of (x - k)^2; then int32
+ * counts[chunks] = pixels of each chunk (the same for every entry; a chunk of 0 pixels has all partials 0), summing to HW.
+ * -> stats [B, Cs, 2] = (mean, rstd).  The finalize adds the chunks in a fixed order in double precision: first the plane mean,
+ * then each chunk's squared deviations from it.  Pivoted partials keep mean and rstd at fp32 accuracy on planes whose mean is
+ * large next to their spread, where (sum, sum of squares) about zero cancels.
+ * Used with vt_conv_desc.stats_ws (partials written by the producing conv). */
 int vt_instnorm_finalize_f32(const float* ws, float* stats, int B, int Cs, int chunks, int64_t HW, float eps, void* stream);
+/* floats of the vt_instnorm_finalize_f32 layout for (chunks, B, Cs): chunks * (B * Cs * 3 + 1); -1 for a non-positive argument */
+int64_t vt_instnorm_partials_floats(int64_t chunks, int B, int Cs);
 /* AdaIN as a per-(sample, channel) affine: affine[b][c] = (gamma*rstd, beta - gamma*mean*rstd); stats [B][Cs][2], gamma_beta [B][2*Cs] */
 int vt_adain_affine_f32(const float* stats, const float* gamma_beta, float* affine, int B, int Cs, void* stream);
 /* out[b,p,c] = gamma[b,c] * (x - mean) * rstd + beta[b,c]; gamma_beta: [B, 2*Cs] (gamma then beta) */

@@ -33,11 +33,11 @@ def test_library_exports_every_declared_symbol():
     assert set(declared) <= set(exported)
 
 
-def test_load_binds_and_reports_version():
+def test_load_binds_and_reports_abi_version():
     from vtoonify_b200 import _lib
     lib = _lib.load()
-    assert lib.vt_abi_version() == _lib.ABI_VERSION == 6
-    assert b"abi=6" in lib.vt_build_info()
+    assert lib.vt_abi_version() == _lib.ABI_VERSION == 7
+    assert b"abi=7" in lib.vt_build_info()
     assert b"sm_90a" in lib.vt_build_info()
     assert ctypes.sizeof(_lib.ConvDesc) % 8 == 0
 
@@ -76,6 +76,12 @@ def test_host_only_entry_points():
     assert b"up/down" in lib.vt_last_error()
     assert lib.vt_instnorm_ws_bytes(4, 72 * 128, 512, 0) > 0
     assert lib.vt_instnorm_ws_bytes(4, 72 * 128, 6, 0) == -1
+    # pivoted partials: (pivot, sum and square sum of x - pivot) per (chunk, b, c) plus one pixel count per chunk;
+    # 72x128 at C = 512 plans 144 chunks of 64 pixels
+    assert lib.vt_instnorm_partials_floats(144, 4, 512) == 144 * (4 * 512 * 3 + 1)
+    assert lib.vt_instnorm_ws_bytes(4, 72 * 128, 512, 0) == 4 * lib.vt_instnorm_partials_floats(144, 4, 512)
+    assert lib.vt_instnorm_ws_bytes(4, 72 * 128, 512, 1) == 4 * lib.vt_instnorm_partials_floats(144, 4, 1024)
+    assert lib.vt_instnorm_partials_floats(0, 4, 512) == -1
     d = _lib.ConvDesc()
     assert lib.vt_conv2d_tc_supported(d) == 0          # wrong struct_size -> rejected without touching the GPU
     assert lib.vt_conv2d_direct_f32(d, None) != 0 and b"size mismatch" in lib.vt_last_error()

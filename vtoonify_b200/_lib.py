@@ -10,7 +10,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvtoonify_b200.so")
-ABI_VERSION = 6
+ABI_VERSION = 7
 VT_MAX_TAPS = 36
 ACT_NONE, ACT_LRELU, ACT_RELU_TANH = 0, 1, 2
 
@@ -103,6 +103,7 @@ SYMBOLS = {
                                 c_float, c_float, c_int, _P]),
     "vt_instnorm_ws_bytes": (c_int64, [c_int, c_int64, c_int, c_int]),
     "vt_instnorm_finalize_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int64, c_float, _P]),
+    "vt_instnorm_partials_floats": (c_int64, [c_int64, c_int, c_int]),
     "vt_conv2d_tc_stats_chunks": (c_int, [POINTER(ConvDesc)]),
     "vt_instnorm_stats_nhwc": (c_int, [_P, _P, c_int, c_int, c_int64, c_int, c_int, c_float, _P, _P, _P]),
     "vt_frame_s2d_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),

@@ -94,8 +94,10 @@ struct TcArgs {
   int mma_n;                 // N of one MMA: block_n, or 2*block_n in the N-stacked bf16x3 form
   int m_major;               // work-item order: the N tiles of one pixel tile are neighbours (run on neighbouring SMs at the same
                              // time, so the second read of the activations hits L2) instead of N-tile-major
-  float* stats_ws;           // optional instance-norm partial sums of the OUTPUT: [chunk][B][Cout][2] (sum, sum of squares), one chunk per
-                             // (pixel tile, consumer warp); finalised by vt_instnorm_finalize_f32
+  float* stats_ws;           // optional instance-norm partials of the OUTPUT in the layout of vt_instnorm_finalize_f32 (pivot,
+                             // deviation sum, square sum about the pivot), one chunk per (pixel tile, consumer warp)
+  int64_t stats_e;           // entries per partial array: chunks * B * Cout
+  int* stats_cnt;            // [chunk] in-image pixels of each chunk (after the three arrays)
   float acc_scale;           // accumulators are multiplied by this first (undoes the power-of-two weight scale of the fp16 split)
 };
 
@@ -496,6 +498,10 @@ __device__ __forceinline__ void conv_tc_body(const TcArgs& p) {
           off0[h] = (int64_t)b * p.out_sb + (int64_t)oy[h] * p.out_sy + (int64_t)ox[h] * p.out_sx;
           pix0[h] = (int64_t)b * p.pix_sb + (int64_t)oy[h] * p.pix_sy + (int64_t)ox[h] * p.pix_sx;   // dense-pixel index
         }
+        // in-image pixels of this warp's 16 (lanes 4r hold pixel row r of both halves h), and 1 / 0 masks of this lane's two
+        const int st_cnt = p.stats_ws ? __popc(__ballot_sync(0xffffffffu, in_img[0]) & 0x11111111u) +
+                                            __popc(__ballot_sync(0xffffffffu, in_img[1]) & 0x11111111u) : 0;
+        const float st_m0 = in_img[0] ? 1.f : 0.f, st_m1 = in_img[1] ? 1.f : 0.f;
         int ph = ph0, nb = nb0 - 32;
 #pragma unroll
         for (int j = 0; j < NW / 32; ++j) {
@@ -557,23 +563,34 @@ __device__ __forceinline__ void conv_tc_body(const TcArgs& p) {
             }
           }
           if (p.stats_ws) {
-            // AdaptiveInstanceNorm statistics of the tensor this launch writes (model/dualstylegan.py:10-21): per channel, the
-            // warp's 16 pixels summed in a fixed butterfly order (no atomics), pixels outside the image masked
+            // AdaptiveInstanceNorm statistics of the tensor this launch writes (model/dualstylegan.py:10-21): per channel over the
+            // warp's in-image pixels, the sum and the sum of squares of x - pivot, both in a fixed butterfly order (no atomics).
+            // The pivot is the chunk's first pixel (lane qd, h = 0: in the image whenever any pixel of the chunk is), so the
+            // finalize's cancellation stays within a factor of the chunk's 16 pixels; about zero, or as an fp32 chunk sum, an
+            // offset plane would lose its variance.  Pixels outside the image hold 0, so x - pivot * mask drops them.
             const int kchunk = ((rem * MT + g) * STATS_WARPS) + half * 4 + tw_;
-            float2* wsp = reinterpret_cast<float2*>(p.stats_ws) + ((int64_t)kchunk * p.B + b) * p.Cout + nb + 2 * qd;
+            // every lane ends with the chunk's values: lanes 4c + qd store component c (pivot, deviation sum, square sum) of
+            // both channels of their pair
+            const int comp = lane >> 2;
+            float2* wsp = reinterpret_cast<float2*>(p.stats_ws + comp * p.stats_e + ((int64_t)kchunk * p.B + b) * p.Cout + nb + 2 * qd);
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
+            for (int k = 0; k < 4; ++k) {
+              float out[2];
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                float ssum = v[0][k][e] + v[1][k][e];
-                float ssq = fmaf(v[0][k][e], v[0][k][e], v[1][k][e] * v[1][k][e]);
+                const float piv = __shfl_sync(0xffffffffu, v[0][k][e], qd);
+                const float d0 = fmaf(-piv, st_m0, v[0][k][e]), d1 = fmaf(-piv, st_m1, v[1][k][e]);
+                float dsum = d0 + d1, dsq = fmaf(d0, d0, d1 * d1);
 #pragma unroll
                 for (int o = 4; o < 32; o <<= 1) {
-                  ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
-                  ssq += __shfl_xor_sync(0xffffffffu, ssq, o);
+                  dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
+                  dsq += __shfl_xor_sync(0xffffffffu, dsq, o);
                 }
-                if (lane < 4) wsp[8 * k + e] = make_float2(ssum, ssq);
+                out[e] = comp == 0 ? piv : (comp == 1 ? dsum : dsq);
               }
+              if (comp < 3) wsp[4 * k] = make_float2(out[0], out[1]);
+            }
+            if (b == 0 && n0 == 0 && j == 0 && lane == 0) p.stats_cnt[kchunk] = st_cnt;
           }
         }
         if (!REALLOC && p.rgb_w) {
@@ -932,10 +949,13 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out, int
     }
     if (d->stats_ws) {
       VT_CHECK(d->n_phase == 1 && !d->rgb_w, "conv_tc: output statistics need one phase and no fused ToRGB");
-      VT_CHECK(d->stats_ws_floats >= chunks * d->B * d->Cout * 2, "conv_tc: stats_ws too small (%lld floats, need %lld)",
-               (long long)d->stats_ws_floats, (long long)(chunks * d->B * d->Cout * 2));
+      const int64_t need = vt_instnorm_partials_floats(chunks, d->B, d->Cout);
+      VT_CHECK(d->stats_ws_floats >= need, "conv_tc: stats_ws too small (%lld floats, need %lld)", (long long)d->stats_ws_floats,
+               (long long)need);
       VT_CHECK(((uintptr_t)d->stats_ws & 7) == 0, "conv_tc: stats_ws not 8-byte aligned");
       a.stats_ws = d->stats_ws;
+      a.stats_e = chunks * d->B * d->Cout;
+      a.stats_cnt = reinterpret_cast<int*>(d->stats_ws + 3 * a.stats_e);
     }
   }
 

@@ -14,14 +14,49 @@ int g_fir4 = 1;   // 1: specialised 4x4 pad (1,1) FIR kernel; 0: generic kernel 
 
 namespace {
 
-// Deterministic two-stage reduction (no atomics): stage 1 — grid (chunks, B): every thread owns one float4 channel
-// group and every pstep-th pixel of its chunk, partials are combined across the pixel lanes in a fixed order through
-// shared memory and written to ws[chunk][b][Cs][2]; stage 2 sums the chunks in index order in double.
-// dyn smem: pstep * Cs * 2 floats.
+// Chan's merge of a group of nk values with sum sk and squared deviations m2k about their own mean into (n, s, m2):
+// n*nk/(n+nk) * (mean_k - mean)^2 written with sums.  Groups are combined this way or, in the finalize, about the known plane mean, so no
+// sum of squares about zero is ever formed: its rounding (u * E[x^2]) would swamp the variance of an offset plane.  An empty
+// group (nk = 0, sk = m2k = 0) changes nothing.
+__device__ __forceinline__ void chan_merge(double& n, double& s, double& m2, double nk, double sk, double m2k) {
+  const double t = nk * s - n * sk;
+  const float den = (float)(n * nk * (n + nk));
+  m2 += (den > 0.f ? t * t * (double)__frcp_rn(den) : 0.0) + m2k;   // a positive term: fp32 reciprocal accuracy is plenty
+  s += sk; n += nk;
+}
+
+// One thread's running statistics of one channel, about a pivot k (the thread's first value): s = sum of (x - k), m2 = squared
+// deviations from the running mean.  Pixels arrive in blocks (a trip of 8 pixels, or the tail pixels) that accumulate
+// (sum, sum of squares) of x - kb, kb = the block's first value: 3 flops per value, and the cancellation in the block's
+// M2 = q - s^2 / nb stays within a factor of the block length (8).  Blocks are merged with Chan's update.
+struct RunStat { float k, s, m2; };
+
+// Weights of merging a block of nb values after n: 1/nb, 1/n (0 for the first block) and n nb / (n + nb); shared by the channels.
+struct MergeW { float inv_nb, inv_n, w; };
+
+__device__ __forceinline__ MergeW merge_weights(float n, float nb) {
+  return MergeW{__frcp_rn(nb), n > 0.f ? __frcp_rn(n) : 0.f, n * nb * __frcp_rn(n + nb)};
+}
+
+// merge a block of nb values (deviation sum bs and square sum bq about its pivot kb) into r; the first block sets the pivot
+__device__ __forceinline__ void run_merge(RunStat& r, float kb, float bs, float bq, float nb, const MergeW& mw) {
+  if (mw.inv_n == 0.f) r.k = kb;
+  const float m2b = fmaxf(fmaf(-bs, bs * mw.inv_nb, bq), 0.f);
+  const float sb = fmaf(nb, kb - r.k, bs);                      // the block's deviation sum about r.k
+  const float delta = sb * mw.inv_nb - r.s * mw.inv_n;
+  r.m2 = fmaf(delta * mw.w, delta, r.m2 + m2b);
+  r.s += sb;
+}
+
+// Deterministic two-stage reduction (no atomics) into the layout of vt_instnorm_finalize_f32: stage 1, grid (chunks, B): every
+// thread owns one float4 channel group and every pstep-th pixel of its chunk; the pixel lanes' (pivot, deviation sum, M2) are
+// merged in lane order through shared memory (Chan, double) into the chunk's entry, and block (chunk, 0) writes the chunk's
+// pixel count.  Stage 2 merges the chunks (instnorm_finalize_kernel).  dyn smem: pstep * Cs * 3 floats.
+template <int mode>
 __global__ void __launch_bounds__(256)
-instnorm_partial_kernel(const float* __restrict__ in, const float* __restrict__ in2, int mode, int64_t HW, int C,
-                        int c_stride, int64_t chunk, float* __restrict__ ws) {
-  extern __shared__ float sacc[];  // [pstep][Cs][2]
+instnorm_partial_kernel(const float* __restrict__ in, const float* __restrict__ in2, int64_t HW, int C, int c_stride, int64_t chunk,
+                        float* __restrict__ ws) {
+  extern __shared__ float sacc[];  // [pstep][Cs][3]
   const int Cs = mode ? 2 * C : C;
   const int b = blockIdx.y;
   const int nvec = C / 4;
@@ -32,91 +67,157 @@ instnorm_partial_kernel(const float* __restrict__ in, const float* __restrict__ 
   const int pstep = blockDim.x / nvec;           // >= 1 (nvec <= 256 checked by the host)
   const int v = threadIdx.x % nvec, lane_p = threadIdx.x / nvec;
   if (lane_p < pstep) {
-    float s[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0}, s2[4] = {0, 0, 0, 0}, q2[4] = {0, 0, 0, 0};
-    // four pixels per trip: the loads are issued together (the kernel is latency-bound: one 16-byte load in flight per thread
-    // gave 1.2 TB/s on L2-resident maps), the accumulation order stays the pixel order
-    int64_t p = p_begin + lane_p;
-    for (; p + 3 * (int64_t)pstep < p_end; p += 4 * (int64_t)pstep) {
-      float4 a[4], e[4];
+    RunStat r[4], r2[4];
 #pragma unroll
-      for (int u = 0; u < 4; ++u) a[u] = __ldg(reinterpret_cast<const float4*>(ip + (p + u * (int64_t)pstep) * c_stride + v * 4));
+    for (int i = 0; i < 4; ++i) r[i] = r2[i] = RunStat{0.f, 0.f, 0.f};
+    float n = 0.f;   // pixels merged so far (exact: < 2^24 per thread)
+    int64_t p = p_begin + lane_p;
+    // eight pixels per trip, one block: the loads are issued together (the kernel is latency-bound: one 16-byte load in flight
+    // per thread gave 1.2 TB/s on L2-resident maps), the accumulation order stays the pixel order
+    for (; p + 7 * (int64_t)pstep < p_end; p += 8 * (int64_t)pstep) {
+      float4 a[8], e[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) a[u] = __ldg(reinterpret_cast<const float4*>(ip + (p + u * (int64_t)pstep) * c_stride + v * 4));
       if (mode) {
 #pragma unroll
-        for (int u = 0; u < 4; ++u) e[u] = __ldg(reinterpret_cast<const float4*>(ip2 + (p + u * (int64_t)pstep) * c_stride + v * 4));
+        for (int u = 0; u < 8; ++u) e[u] = __ldg(reinterpret_cast<const float4*>(ip2 + (p + u * (int64_t)pstep) * c_stride + v * 4));
+      }
+      const float kb[4] = {a[0].x, a[0].y, a[0].z, a[0].w};
+      float kb2[4], bs[4] = {0, 0, 0, 0}, bq[4] = {0, 0, 0, 0}, bs2[4] = {0, 0, 0, 0}, bq2[4] = {0, 0, 0, 0};
+      if (mode) {
+        kb2[0] = fabsf(a[0].x - e[0].x); kb2[1] = fabsf(a[0].y - e[0].y); kb2[2] = fabsf(a[0].z - e[0].z); kb2[3] = fabsf(a[0].w - e[0].w);
       }
 #pragma unroll
-      for (int u = 0; u < 4; ++u) {
+      for (int u = 0; u < 8; ++u) {
         const float av[4] = {a[u].x, a[u].y, a[u].z, a[u].w};
 #pragma unroll
-        for (int i = 0; i < 4; ++i) { s[i] += av[i]; q[i] = fmaf(av[i], av[i], q[i]); }
+        for (int i = 0; i < 4; ++i) { const float d = av[i] - kb[i]; bs[i] += d; bq[i] = fmaf(d, d, bq[i]); }
         if (mode) {
           const float ev[4] = {e[u].x, e[u].y, e[u].z, e[u].w};
 #pragma unroll
-          for (int i = 0; i < 4; ++i) { const float d = fabsf(av[i] - ev[i]); s2[i] += d; q2[i] = fmaf(d, d, q2[i]); }
+          for (int i = 0; i < 4; ++i) { const float d = fabsf(av[i] - ev[i]) - kb2[i]; bs2[i] += d; bq2[i] = fmaf(d, d, bq2[i]); }
         }
       }
-    }
-    for (; p < p_end; p += pstep) {
-      const float4 a = *reinterpret_cast<const float4*>(ip + p * c_stride + v * 4);
-      const float av[4] = {a.x, a.y, a.z, a.w};
+      const MergeW mw = merge_weights(n, 8.f);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) { s[i] += av[i]; q[i] = fmaf(av[i], av[i], q[i]); }
-      if (mode) {
-        const float4 e = *reinterpret_cast<const float4*>(ip2 + p * c_stride + v * 4);
-        const float ev[4] = {e.x, e.y, e.z, e.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { const float d = fabsf(av[i] - ev[i]); s2[i] += d; q2[i] = fmaf(d, d, q2[i]); }
+      for (int i = 0; i < 4; ++i) {
+        run_merge(r[i], kb[i], bs[i], bq[i], 8.f, mw);
+        if (mode) run_merge(r2[i], kb2[i], bs2[i], bq2[i], 8.f, mw);
       }
+      n += 8.f;
     }
-    float* row = sacc + (size_t)lane_p * Cs * 2;
+    if (p < p_end) {   // the tail: fewer than 8 pixels of this lane left, one block
+      float kb[4], kb2[4], bs[4] = {0, 0, 0, 0}, bq[4] = {0, 0, 0, 0}, bs2[4] = {0, 0, 0, 0}, bq2[4] = {0, 0, 0, 0};
+      float nb = 0.f;
+      for (; p < p_end; p += pstep) {
+        const float4 a = *reinterpret_cast<const float4*>(ip + p * c_stride + v * 4);
+        const float av[4] = {a.x, a.y, a.z, a.w};
+        float ev[4] = {0, 0, 0, 0};
+        if (mode) {
+          const float4 e = *reinterpret_cast<const float4*>(ip2 + p * c_stride + v * 4);
+          ev[0] = fabsf(a.x - e.x); ev[1] = fabsf(a.y - e.y); ev[2] = fabsf(a.z - e.z); ev[3] = fabsf(a.w - e.w);
+        }
+        if (nb == 0.f) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) { kb[i] = av[i]; kb2[i] = ev[i]; }
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float d = av[i] - kb[i]; bs[i] += d; bq[i] = fmaf(d, d, bq[i]);
+          if (mode) { const float d2 = ev[i] - kb2[i]; bs2[i] += d2; bq2[i] = fmaf(d2, d2, bq2[i]); }
+        }
+        nb += 1.f;
+      }
+      const MergeW mw = merge_weights(n, nb);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        run_merge(r[i], kb[i], bs[i], bq[i], nb, mw);
+        if (mode) run_merge(r2[i], kb2[i], bs2[i], bq2[i], nb, mw);
+      }
+      n += nb;
+    }
+    float* row = sacc + (size_t)lane_p * Cs * 3;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      row[(v * 4 + i) * 2 + 0] = s[i];
-      row[(v * 4 + i) * 2 + 1] = q[i];
+      float* e = row + (v * 4 + i) * 3;
+      e[0] = r[i].k; e[1] = r[i].s; e[2] = r[i].m2;
       if (mode) {
-        row[(C + v * 4 + i) * 2 + 0] = s2[i];
-        row[(C + v * 4 + i) * 2 + 1] = q2[i];
+        e = row + (C + v * 4 + i) * 3;
+        e[0] = r2[i].k; e[1] = r2[i].s; e[2] = r2[i].m2;
       }
     }
   }
   __syncthreads();
-  float* wrow = ws + ((int64_t)blockIdx.x * gridDim.y + b) * Cs * 2;
-  for (int i = threadIdx.x; i < Cs * 2; i += blockDim.x) {
-    float t = 0.f;
-    for (int l = 0; l < pstep; ++l) t += sacc[(size_t)l * Cs * 2 + i];
-    wrow[i] = t;
+  const int span = (int)(p_end - p_begin);   // < 2^24 (host check)
+  const int64_t E = (int64_t)gridDim.x * gridDim.y * Cs, e0 = ((int64_t)blockIdx.x * gridDim.y + b) * Cs;
+  for (int i = threadIdx.x; i < Cs; i += blockDim.x) {
+    double n = 0.0, s = 0.0, m2 = 0.0;
+    for (int l = 0; l < pstep && l < span; ++l) {   // lane l holds pixels p_begin + l, + pstep, ... of the chunk
+      const float* e = sacc + ((size_t)l * Cs + i) * 3;
+      const double nl = (double)((unsigned)(span - l + pstep - 1) / (unsigned)pstep);
+      chan_merge(n, s, m2, nl, nl * e[0] + e[1], e[2]);
+    }
+    // pivot on the chunk mean rounded to fp32: the deviation sum keeps the rest of the mean, and the square sum about the pivot
+    // is M2 plus a term of the size of that rounding
+    const float k0 = (float)(s / n);
+    const double dev = s - n * k0;
+    ws[e0 + i] = k0;
+    ws[E + e0 + i] = (float)dev;
+    ws[2 * E + e0 + i] = (float)(m2 + dev * dev / n);
   }
+  if (b == 0 && threadIdx.x == 0) reinterpret_cast<int*>(ws + 3 * E)[blockIdx.x] = span;
 }
 
-// block = 32 (b, c) entries x 8 chunk slices: slice ks adds chunks ks, ks + 8, ... in double, the 8 slice sums are then added in
-// slice order (fixed order -> deterministic).  One thread per entry walking all chunks was a 140-step dependent chain of
-// strided loads (57 us per call on the 72x128 maps once the partial kernel went to 144 chunks).
+// block = 8 (b, c) entries x 32 chunk slices, two passes over the chunks (fixed order -> deterministic): slice ks adds the pixel
+// counts and sums of chunks ks, ks + 32, ... in double, the 32 slice results are added in slice order into the plane mean; then
+// slice ks adds each chunk's squared deviations from that mean, q_k + 2 (k - mean) d_k + n_k (k - mean)^2 for the chunk's pivot k,
+// deviation sum d_k and square sum q_k about k, the same way.  Every addend of a pass is independent of the others
+// (a Chan merge per chunk would chain a dozen dependent operations per step), so the loads stay in flight.  One thread per
+// entry walking all chunks was a 140-step dependent chain of strided loads (57 us per call on the 72x128 maps once the
+// partial kernel went to 144 chunks).
+constexpr int FIN_ENTRIES = 8, FIN_SLICES = 32;   // 256 threads; more slices keep more SMs busy on few (b, c) entries
+
 __global__ void __launch_bounds__(256)
 instnorm_finalize_kernel(const float* __restrict__ ws, float* __restrict__ stats, int n, int chunks, double inv_hw, float eps) {
-  __shared__ double red[2][8][32];
-  const int li = threadIdx.x & 31, ks = threadIdx.x >> 5;
-  const int i = blockIdx.x * 32 + li;   // i = b * Cs + c
-  double s = 0.0, q = 0.0;
+  __shared__ double red[3][FIN_SLICES][FIN_ENTRIES];
+  const int li = threadIdx.x % FIN_ENTRIES, ks = threadIdx.x / FIN_ENTRIES;
+  const int i = blockIdx.x * FIN_ENTRIES + li;   // i = b * Cs + c
+  const int64_t E = (int64_t)chunks * n;
+  const int* cnt = reinterpret_cast<const int*>(ws + 3 * E);
+  double c = 0.0, s = 0.0;
   if (i < n) {
-    const float2* w2 = reinterpret_cast<const float2*>(ws);
 #pragma unroll 4
-    for (int k = ks; k < chunks; k += 8) {
-      const float2 v = __ldg(w2 + (int64_t)k * n + i);
-      s += (double)v.x;
-      q += (double)v.y;
+    for (int k = ks; k < chunks; k += FIN_SLICES) {
+      const double ck = (double)__ldg(cnt + k);
+      const int64_t j = (int64_t)k * n + i;
+      c += ck;
+      s += ck * __ldg(ws + j) + __ldg(ws + E + j);
     }
   }
-  red[0][ks][li] = s; red[1][ks][li] = q;
+  red[0][ks][li] = c; red[1][ks][li] = s;
+  __syncthreads();
+  double cc = 0.0, ss = 0.0;
+#pragma unroll
+  for (int k = 0; k < FIN_SLICES; ++k) { cc += red[0][k][li]; ss += red[1][k][li]; }
+  const double mean = cc > 0.0 ? ss / cc : 0.0;
+  double q = 0.0;
+  if (i < n) {
+#pragma unroll 4
+    for (int k = ks; k < chunks; k += FIN_SLICES) {
+      const double ck = (double)__ldg(cnt + k);
+      const int64_t j = (int64_t)k * n + i;
+      const double a = (double)__ldg(ws + j) - mean;   // a chunk of no pixels has all partials 0 and adds 0
+      q += __ldg(ws + 2 * E + j) + a * (2.0 * __ldg(ws + E + j) + ck * a);
+    }
+  }
+  red[2][ks][li] = q;
   __syncthreads();
   if (ks == 0 && i < n) {
-    double ss = 0.0, qq = 0.0;
+    double qq = 0.0;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) { ss += red[0][k][li]; qq += red[1][k][li]; }
-    const double mean = ss * inv_hw;
-    double var = qq * inv_hw - mean * mean;
-    if (var < 0) var = 0;
-    stats[i * 2] = (float)mean;
-    stats[i * 2 + 1] = (float)(1.0 / sqrt(var + (double)eps));
+    for (int k = 0; k < FIN_SLICES; ++k) qq += red[2][k][li];
+    stats[i * 2] = (float)(ss * inv_hw);
+    stats[i * 2 + 1] = (float)(1.0 / sqrt(fmax(qq, 0.0) * inv_hw + (double)eps));
   }
 }
 
@@ -339,11 +440,16 @@ static void instnorm_plan(int64_t HW, int C, int64_t* chunk, int64_t* chunks) {
   *chunks = vt_cdiv(HW, ch);
 }
 
+extern "C" int64_t vt_instnorm_partials_floats(int64_t chunks, int B, int Cs) {
+  if (chunks < 1 || B < 1 || Cs < 1) return -1;
+  return chunks * ((int64_t)B * Cs * 3 + 1);
+}
+
 extern "C" int64_t vt_instnorm_ws_bytes(int B, int64_t HW, int C, int mode) {
   if (B < 1 || HW < 1 || C < 4 || C % 4 || C / 4 > 256) return -1;
   int64_t chunk, chunks;
   instnorm_plan(HW, C, &chunk, &chunks);
-  return chunks * B * (mode ? 2 * C : C) * 2 * (int64_t)sizeof(float);
+  return vt_instnorm_partials_floats(chunks, B, mode ? 2 * C : C) * (int64_t)sizeof(float);
 }
 
 extern "C" int vt_instnorm_stats_nhwc(const float* in, const float* in2, int mode, int B, int64_t HW, int C, int c_stride,
@@ -355,13 +461,15 @@ extern "C" int vt_instnorm_stats_nhwc(const float* in, const float* in2, int mod
   cudaStream_t st = (cudaStream_t)stream;
   int64_t chunk, chunks;
   instnorm_plan(HW, C, &chunk, &chunks);
+  VT_CHECK(chunk < (1LL << 24) && chunks < (1LL << 31), "instnorm_stats: plane too large (%lld pixels)", (long long)HW);
   const int pstep = 256 / (C / 4);
   dim3 grid((unsigned)chunks, (unsigned)B);
-  instnorm_partial_kernel<<<grid, 256, (size_t)pstep * Cs * 2 * sizeof(float), st>>>(in, in2, mode, HW, C, c_stride, chunk,
-                                                                                    (float*)ws);
+  const size_t smem = (size_t)pstep * Cs * 3 * sizeof(float);
+  if (mode) instnorm_partial_kernel<1><<<grid, 256, smem, st>>>(in, in2, HW, C, c_stride, chunk, (float*)ws);
+  else instnorm_partial_kernel<0><<<grid, 256, smem, st>>>(in, in2, HW, C, c_stride, chunk, (float*)ws);
   VT_LAUNCH_CHECK();
   const int n = B * Cs;
-  instnorm_finalize_kernel<<<(unsigned)vt_cdiv(n, 32), 256, 0, st>>>((const float*)ws, stats, n, (int)chunks,
+  instnorm_finalize_kernel<<<(unsigned)vt_cdiv(n, FIN_ENTRIES), 256, 0, st>>>((const float*)ws, stats, n, (int)chunks,
                                                                     1.0 / (double)HW, eps);
   VT_LAUNCH_CHECK();
   return 0;
@@ -370,7 +478,7 @@ extern "C" int vt_instnorm_stats_nhwc(const float* in, const float* in2, int mod
 extern "C" int vt_instnorm_finalize_f32(const float* ws, float* stats, int B, int Cs, int chunks, int64_t HW, float eps, void* stream) {
   VT_CHECK(ws && stats && B >= 1 && Cs >= 1 && chunks >= 1 && HW >= 1, "instnorm_finalize: bad args");
   const int n = B * Cs;
-  instnorm_finalize_kernel<<<(unsigned)vt_cdiv(n, 32), 256, 0, (cudaStream_t)stream>>>(ws, stats, n, chunks, 1.0 / (double)HW, eps);
+  instnorm_finalize_kernel<<<(unsigned)vt_cdiv(n, FIN_ENTRIES), 256, 0, (cudaStream_t)stream>>>(ws, stats, n, chunks, 1.0 / (double)HW, eps);
   VT_LAUNCH_CHECK();
   return 0;
 }

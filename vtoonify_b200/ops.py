@@ -397,7 +397,7 @@ def conv2d_nhwc(srcs: Sequence[torch.Tensor], weight: torch.Tensor, taps, stride
     """General NHWC convolution (virtual channel-concat of ``srcs``).
 
     ``want_stats``: also return the instance-norm statistics ``[B, Cout, 2]`` = (mean, rstd) of the OUTPUT (what
-    :func:`instnorm_stats` would compute from it): the tensor-core kernel's epilogue warps write per-tile partial sums of the values
+    :func:`instnorm_stats` would compute from it): the tensor-core kernel's epilogue warps write per-tile centred partials of the values
     they store and only the finalize pass runs afterwards; other routes fall back to the separate statistics pass.
 
     ``weight``: ``[wB, w_taps, Cout, w_cstride]`` from :func:`prep_weights`.
@@ -518,7 +518,7 @@ def conv2d_nhwc(srcs: Sequence[torch.Tensor], weight: torch.Tensor, taps, stride
             raise _lib.VtError("conv2d_nhwc: want_stats needs a dense single-phase output without the fused ToRGB tail")
         chunks = lib.vt_conv2d_tc_stats_chunks(d) if (use_tc and _options["fuse_stats"]) else -1
         if chunks > 0:
-            stats_ws = torch.empty((chunks * B * Cout * 2,), device=out.device, dtype=torch.float32)
+            stats_ws = torch.empty((lib.vt_instnorm_partials_floats(chunks, B, Cout),), device=out.device, dtype=torch.float32)
             d.stats_ws, d.stats_ws_floats = stats_ws.data_ptr(), stats_ws.numel()
     if use_tc:
         if _tc_profile is not None:

@@ -315,6 +315,22 @@ int vt_adain_affine_f32(const float* stats, const float* gamma_beta, float* affi
 int vt_adain_apply_nhwc(const float* in, const float* in2, int mode, int B, int64_t HW, int C, int c_stride,
                         const float* stats, const float* gamma_beta, float* out, int round_tf32, void* stream);
 
+/* ---- backward of the encoder path (NHWC [B, HW, C], C % 4 == 0, C <= 1024, 16-byte aligned tensors) --------------------- */
+/* Both entry points follow the chunk plan of vt_instnorm_stats_nhwc (it depends on (HW, C) only) and reduce without atomics in
+ * a fixed order, in double precision: the same inputs give bit-identical results.  ws: vt_act_grad_ws_bytes(B, HW, C) bytes. */
+int64_t vt_act_grad_ws_bytes(int B, int64_t HW, int C);
+/* Reduction half of the instance-norm backward: sums[b][c] = (sum_p g, sum_p g * xhat), xhat = (x - mean) * rstd with the
+ * statistics the forward applied (stats [B][C][2] = (mean, rstd)).  The two sums are also dbeta and dgamma of the affine. */
+int vt_adain_grad_stats_nhwc(const float* g, const float* x, const float* stats, int B, int64_t HW, int C, float* sums,
+                             void* ws, void* stream);
+/* Elementwise half: out = beta * res + gate(ref) * gain * T(g), gate(ref) = ref > 0 ? 1 : slope (ref NULL: 1), res may be NULL.
+ * T(g) = g when x is NULL; otherwise the AdaIN backward gamma * rstd * ((g - m_g) - (x - mean) * rstd * m_gx) with
+ * m_g, m_gx = sums / HW from vt_adain_grad_stats_nhwc and gamma from gamma_beta [B][2C] (gamma then beta).
+ * bias_grad (may be NULL): [C] = sum over b and p of out, from per-chunk partials of the same pass. */
+int vt_act_grad_nhwc(const float* g, const float* ref, float slope, float gain, const float* res, float beta, const float* x,
+                     const float* stats, const float* gamma_beta, const float* sums, int B, int64_t HW, int C, float* out,
+                     float* bias_grad, void* ws, void* stream);
+
 /* ---- pSp encoder helpers (model/encoder/encoders/helpers.py:56-119, psp_encoders.py:72-88) ---------------- */
 /* out[b,y,x,c] = x[b,y,x,c] * gate[b,c] + sc[b, y*sc_stride, x*sc_stride, c]   (SE gate + shortcut add; gate may be NULL = 1,
  * sc: NHWC [B, Hs, Ws, C] with Hs >= (H-1)*sc_stride+1; MaxPool2d(1, stride) shortcut == strided sampling) */

@@ -546,3 +546,210 @@ extern "C" int vt_fir_nhwc_f32(const float* in, const float* kernel, float* out,
   VT_LAUNCH_CHECK();
   return 0;
 }
+
+// ---- backward of the encoder path (VToonify.forward(return_feat=True) under autograd) -------------------------------------
+//   vt_adain_grad_stats_nhwc : per (b, c) the sums of g and of g * xhat, xhat = (x - mean) * rstd with the saved statistics
+//   vt_act_grad_nhwc         : out = beta * res + gate(ref) * gain * T(g), T = identity or the AdaIN backward, and optionally the
+//                              per-channel sums of out (a bias gradient) in the same pass
+// Both walk the maps with the chunk plan of the statistics pass (instnorm_plan: it depends on (HW, C) only) and reduce without
+// atomics: every block writes double partials for its (chunk, sample), a warp per output entry adds them in a fixed order.
+namespace {
+
+// per (chunk, b, c): (sum g, sum g * xhat) in double.  dyn smem: pstep * C * 2 doubles
+__global__ void __launch_bounds__(256)
+adain_grad_partial_kernel(const float* __restrict__ g, const float* __restrict__ x, const float* __restrict__ stats, int64_t HW,
+                          int C, int64_t chunk, double* __restrict__ ws) {
+  extern __shared__ double sred[];
+  const int b = blockIdx.y, nvec = C / 4, pstep = blockDim.x / nvec;
+  const int v = threadIdx.x % nvec, lane_p = threadIdx.x / nvec;
+  const int64_t p_begin = (int64_t)blockIdx.x * chunk;
+  const int64_t p_end = (p_begin + chunk < HW) ? p_begin + chunk : HW;
+  if (lane_p < pstep) {
+    float mean[4], rstd[4];
+    double sg[4] = {0, 0, 0, 0}, sgx[4] = {0, 0, 0, 0};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      mean[i] = stats[((int64_t)b * C + v * 4 + i) * 2];
+      rstd[i] = stats[((int64_t)b * C + v * 4 + i) * 2 + 1];
+    }
+    const float* gp = g + (int64_t)b * HW * C + v * 4;
+    const float* xp = x + (int64_t)b * HW * C + v * 4;
+#pragma unroll 4
+    for (int64_t p = p_begin + lane_p; p < p_end; p += pstep) {
+      const float4 gv = __ldg(reinterpret_cast<const float4*>(gp + p * C));
+      const float4 xv = __ldg(reinterpret_cast<const float4*>(xp + p * C));
+      const float ga[4] = {gv.x, gv.y, gv.z, gv.w}, xa[4] = {xv.x, xv.y, xv.z, xv.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float xh = (xa[i] - mean[i]) * rstd[i];
+        sg[i] += (double)ga[i];
+        sgx[i] = fma((double)ga[i], (double)xh, sgx[i]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      sred[((int64_t)lane_p * C + v * 4 + i) * 2] = sg[i];
+      sred[((int64_t)lane_p * C + v * 4 + i) * 2 + 1] = sgx[i];
+    }
+  }
+  __syncthreads();
+  double* dst = ws + ((int64_t)blockIdx.x * gridDim.y + b) * C * 2;
+  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
+    double s = 0.0;
+    for (int l = 0; l < pstep; ++l) s += sred[(int64_t)l * C * 2 + i];
+    dst[i] = s;
+  }
+}
+
+// out = beta * res + gate(ref) * gain * T(g); T(g) = g, or with ADAIN gamma * rstd * ((g - m_g) - (x - mean) * rstd * m_gx)
+// (m_g, m_gx = plane means of g and g * xhat).  With ws: per (chunk, b, c) the double sum of out.  dyn smem: pstep * C doubles
+template <bool ADAIN>
+__global__ void __launch_bounds__(256)
+act_grad_kernel(const float* __restrict__ g, const float* __restrict__ ref, float slope, float gain, const float* __restrict__ res,
+                float beta, const float* __restrict__ x, const float* __restrict__ stats, const float* __restrict__ gb,
+                const float* __restrict__ sums, float inv_hw, int64_t HW, int C, int64_t chunk, float* __restrict__ out,
+                double* __restrict__ ws) {
+  extern __shared__ double sred[];
+  const int b = blockIdx.y, nvec = C / 4, pstep = blockDim.x / nvec;
+  const int v = threadIdx.x % nvec, lane_p = threadIdx.x / nvec;
+  const int64_t p_begin = (int64_t)blockIdx.x * chunk;
+  const int64_t p_end = (p_begin + chunk < HW) ? p_begin + chunk : HW;
+  if (lane_p < pstep) {
+    float mean[4] = {0, 0, 0, 0}, rstd[4] = {0, 0, 0, 0}, coef[4] = {0, 0, 0, 0}, mg[4] = {0, 0, 0, 0}, mgx[4] = {0, 0, 0, 0};
+    if (ADAIN) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int64_t e = (int64_t)b * C + v * 4 + i;
+        mean[i] = stats[e * 2];
+        rstd[i] = stats[e * 2 + 1];
+        coef[i] = gb[(int64_t)b * 2 * C + v * 4 + i] * rstd[i];
+        mg[i] = sums[e * 2] * inv_hw;
+        mgx[i] = sums[e * 2 + 1] * inv_hw;
+      }
+    }
+    double bs[4] = {0, 0, 0, 0};
+    const int64_t base = (int64_t)b * HW * C + v * 4;
+    for (int64_t p = p_begin + lane_p; p < p_end; p += pstep) {
+      const int64_t o = base + p * C;
+      const float4 gv = __ldg(reinterpret_cast<const float4*>(g + o));
+      float t[4] = {gv.x, gv.y, gv.z, gv.w};
+      if (ADAIN) {
+        const float4 xv = __ldg(reinterpret_cast<const float4*>(x + o));
+        const float xa[4] = {xv.x, xv.y, xv.z, xv.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) t[i] = coef[i] * ((t[i] - mg[i]) - (xa[i] - mean[i]) * rstd[i] * mgx[i]);
+      }
+      if (ref) {
+        const float4 rv = __ldg(reinterpret_cast<const float4*>(ref + o));
+        const float ra[4] = {rv.x, rv.y, rv.z, rv.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) t[i] = ra[i] > 0.f ? t[i] : t[i] * slope;
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) t[i] *= gain;
+      if (res) {
+        const float4 sv = __ldg(reinterpret_cast<const float4*>(res + o));
+        const float sa[4] = {sv.x, sv.y, sv.z, sv.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) t[i] = fmaf(beta, sa[i], t[i]);
+      }
+      *reinterpret_cast<float4*>(out + o) = make_float4(t[0], t[1], t[2], t[3]);
+      if (ws) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) bs[i] += (double)t[i];
+      }
+    }
+    if (ws) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) sred[(int64_t)lane_p * C + v * 4 + i] = bs[i];
+    }
+  }
+  if (!ws) return;
+  __syncthreads();
+  double* dst = ws + ((int64_t)blockIdx.x * gridDim.y + b) * C;
+  for (int i = threadIdx.x; i < C; i += blockDim.x) {
+    double s = 0.0;
+    for (int l = 0; l < pstep; ++l) s += sred[(int64_t)l * C + i];
+    dst[i] = s;
+  }
+}
+
+// out[e] = scale * sum over parts of ws[part * n + e], one warp per entry: lane-strided sums, then a fixed shuffle tree
+__global__ void __launch_bounds__(256)
+partials_sum_kernel(const double* __restrict__ ws, int64_t parts, int64_t n, float scale, float* __restrict__ out) {
+  const int64_t e = (int64_t)blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+  const int lane = threadIdx.x % 32;
+  if (e >= n) return;
+  double s = 0.0;
+  for (int64_t k = lane; k < parts; k += 32) s += __ldg(ws + k * n + e);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) out[e] = (float)(s * (double)scale);
+}
+
+bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+}  // namespace
+
+extern "C" int64_t vt_act_grad_ws_bytes(int B, int64_t HW, int C) {
+  if (B < 1 || HW < 1 || C < 4 || C % 4 || C / 4 > 256) return -1;
+  int64_t chunk, chunks;
+  instnorm_plan(HW, C, &chunk, &chunks);
+  return chunks * B * C * 2 * (int64_t)sizeof(double);
+}
+
+#define VT_GRAD_SHAPE_CHECK(name)                                                                                      \
+  VT_CHECK(B >= 1 && B <= 65535 && HW >= 1 && C >= 4 && C % 4 == 0 && C / 4 <= 256, name ": bad shape (C must be a "   \
+           "multiple of 4, at most 1024)")
+
+extern "C" int vt_adain_grad_stats_nhwc(const float* g, const float* x, const float* stats, int B, int64_t HW, int C,
+                                        float* sums, void* ws, void* stream) {
+  VT_CHECK(g && x && stats && sums && ws, "adain_grad_stats: null pointer");
+  VT_CHECK(aligned16(g) && aligned16(x) && aligned16(ws), "adain_grad_stats: g, x and ws must be 16-byte aligned");
+  VT_GRAD_SHAPE_CHECK("adain_grad_stats");
+  int64_t chunk, chunks;
+  instnorm_plan(HW, C, &chunk, &chunks);
+  VT_CHECK(chunks < (1LL << 31), "adain_grad_stats: plane too large");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int pstep = 256 / (C / 4);
+  adain_grad_partial_kernel<<<dim3((unsigned)chunks, (unsigned)B), 256, (size_t)pstep * C * 2 * sizeof(double), st>>>(
+      g, x, stats, HW, C, chunk, (double*)ws);
+  VT_LAUNCH_CHECK();
+  const int64_t n = (int64_t)B * C * 2;
+  partials_sum_kernel<<<(unsigned)vt_cdiv(n, 8), 256, 0, st>>>((const double*)ws, chunks, n, 1.f, sums);
+  VT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int vt_act_grad_nhwc(const float* g, const float* ref, float slope, float gain, const float* res, float beta,
+                                const float* x, const float* stats, const float* gamma_beta, const float* sums, int B, int64_t HW,
+                                int C, float* out, float* bias_grad, void* ws, void* stream) {
+  VT_CHECK(g && out, "act_grad: null pointer");
+  const bool adain = x != nullptr;
+  VT_CHECK(!adain || (stats && gamma_beta && sums), "act_grad: the AdaIN form needs x, stats, gamma_beta and sums");
+  VT_CHECK(!bias_grad || ws, "act_grad: bias_grad needs ws");
+  VT_CHECK(aligned16(g) && aligned16(out) && (!ref || aligned16(ref)) && (!res || aligned16(res)) && (!x || aligned16(x)) &&
+           (!ws || aligned16(ws)), "act_grad: tensors must be 16-byte aligned");
+  VT_GRAD_SHAPE_CHECK("act_grad");
+  int64_t chunk, chunks;
+  instnorm_plan(HW, C, &chunk, &chunks);
+  VT_CHECK(chunks < (1LL << 31), "act_grad: plane too large");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int pstep = 256 / (C / 4);
+  double* part = bias_grad ? (double*)ws : nullptr;
+  const size_t smem = part ? (size_t)pstep * C * sizeof(double) : 0;
+  const dim3 grid((unsigned)chunks, (unsigned)B);
+  const float inv_hw = (float)(1.0 / (double)HW);
+  if (adain)
+    act_grad_kernel<true><<<grid, 256, smem, st>>>(g, ref, slope, gain, res, beta, x, stats, gamma_beta, sums, inv_hw, HW, C,
+                                                   chunk, out, part);
+  else
+    act_grad_kernel<false><<<grid, 256, smem, st>>>(g, ref, slope, gain, res, beta, x, stats, gamma_beta, sums, inv_hw, HW, C,
+                                                    chunk, out, part);
+  VT_LAUNCH_CHECK();
+  if (bias_grad) {
+    partials_sum_kernel<<<(unsigned)vt_cdiv(C, 8), 256, 0, st>>>(part, chunks * B, C, 1.f, bias_grad);
+    VT_LAUNCH_CHECK();
+  }
+  return 0;
+}

@@ -179,7 +179,25 @@ def _conv_transpose2d_forward(input, weight, bias, s, p, op, d, groups):
     if cpad != Cout:
         w5 = torch.cat([w5, w5.new_zeros((groups, cpad - Cout, Cin, kh, kw))], dim=1)
     w = _prep_grouped(w5.contiguous(), x.shape[3]) if groups > 1 else ops.prep_weights(w5[0].contiguous(), cin_pad=x.shape[3])
-    y = torch.empty((B, Ho, Wo, cpad), device=x.device, dtype=torch.float32)
+    y = conv_transpose_nhwc(x, w, kh, kw, st, p, d, Ho, Wo)
+    out = ops.to_nchw(y, Cout)
+    if groups > 1:
+        out = out.reshape(1, groups * Cout, Ho, Wo)
+    if bias is not None:
+        out = ops.fused_bias_act(out, bias, 1.0, 1.0)
+    return out
+
+
+def conv_transpose_nhwc(x, w, kh, kw, st, p, d, Ho, Wo, res=None, beta=1.0):
+    """The NHWC core of the transposed op: ``x`` [B, H, W, cin_pad], ``w`` [wB, kh*kw, Cout, cin_pad] from ``prep_weights`` of the
+    [Cout, Cin, kh, kw] view of a transposed-conv weight (slab ky*kw + kx, not flipped) -> [B, Ho, Wo, Cout].  One stride-1
+    convolution per output phase (py, px) writes the strided view y[:, py::st, px::st]: output row o = st*j + py receives input row
+    j + (py + pad - ky*dil) / st through tap ky wherever that division is exact.  ``res`` (stride 1 only): ``beta * res`` is
+    added in the convolution's epilogue."""
+    B, cout = x.shape[0], w.shape[2]
+    if res is not None and st != 1:
+        raise NotImplementedError("conv_transpose_nhwc: a residual needs stride 1")
+    y = torch.empty((B, Ho, Wo, cout), device=x.device, dtype=torch.float32)
     for py in range(st):
         for px in range(st):
             Hp, Wp = (Ho - py + st - 1) // st, (Wo - px + st - 1) // st
@@ -191,14 +209,19 @@ def _conv_transpose2d_forward(input, weight, bias, s, p, op, d, groups):
             if not taps:
                 y[:, py::st, px::st].zero_()
                 continue
-            view = ((py * Wo + px) * cpad, Ho * Wo * cpad, st * Wo * cpad, st * cpad)
-            ops.conv2d_nhwc([x], w, taps, 1, Hp, Wp, out=y, out_view=view)
-    out = ops.to_nchw(y, Cout)
-    if groups > 1:
-        out = out.reshape(1, groups * Cout, Ho, Wo)
-    if bias is not None:
-        out = ops.fused_bias_act(out, bias, 1.0, 1.0)
-    return out
+            if st == 1:
+                ops.conv2d_nhwc([x], w, taps, 1, Hp, Wp, out=y, res=res, beta=beta)
+            else:
+                view = ((py * Wo + px) * cout, Ho * Wo * cout, st * Wo * cout, st * cout)
+                ops.conv2d_nhwc([x], w, taps, 1, Hp, Wp, out=y, out_view=view)
+    return y
+
+
+def weight_grad_nhwc(a, src, M, N, kh, kw, s, p, d, per_sample=False):
+    """Weight gradient of a convolution with stride ``s``, padding ``p`` and dilation ``d`` on NHWC operands (channel strides that
+    are multiples of 32): ``a`` holds the M output-side channels, ``src`` the N input-side ones -> [nb * M, N, kh*kw]."""
+    taps = [(ky * d[0] - p[0], kx * d[1] - p[1]) for ky in range(kh) for kx in range(kw)]
+    return ops.conv_wgrad_nhwc(a, src, M, N, taps, s, per_sample)
 
 
 def _weight_grad(transpose, weight_shape, grad_output, input, s, p, d, groups):
@@ -211,8 +234,7 @@ def _weight_grad(transpose, weight_shape, grad_output, input, s, p, d, groups):
     M, N = a4.shape[1], s4.shape[1]
     a = ops.to_nhwc(a4, ops._pad32(M), round_tf32=False)
     src = ops.to_nhwc(s4, ops._pad32(N), round_tf32=False)
-    taps = [(ky * d[0] - p[0], kx * d[1] - p[1]) for ky in range(kh) for kx in range(kw)]
-    return ops.conv_wgrad_nhwc(a, src, M, N, taps, s[0], groups > 1).reshape(weight_shape)
+    return weight_grad_nhwc(a, src, M, N, kh, kw, s[0], p, d, groups > 1).reshape(weight_shape)
 
 
 class _ChannelSum(Function):

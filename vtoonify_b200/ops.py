@@ -826,6 +826,56 @@ def adain_apply(x: torch.Tensor, stats: torch.Tensor, gamma_beta: torch.Tensor, 
     return out
 
 
+def _grad_ws(B: int, HW: int, C: int, device) -> torch.Tensor:
+    nbytes = _lib.load().vt_act_grad_ws_bytes(B, HW, C)
+    if nbytes < 0:
+        raise _lib.VtError(f"act_grad: unsupported shape C={C}")
+    return torch.empty((nbytes // 8,), device=device, dtype=torch.float64)
+
+
+def _nhwc_check(name, ref, *ts):
+    for t in ts:
+        if t is not None and (t.shape != ref.shape or not t.is_contiguous()):
+            raise _lib.VtError(f"{name}: tensors must be contiguous NHWC of the same shape")
+
+
+def adain_grad_stats(g: torch.Tensor, x: torch.Tensor, stats: torch.Tensor) -> torch.Tensor:
+    """Reduction half of the instance-norm backward: ``[B, C, 2]`` = (sum of g, sum of g * xhat) per plane, xhat = (x - mean) * rstd
+    with the statistics ``stats`` [B, C, 2] the forward applied (deterministic, double-precision reduction)."""
+    _req_cuda(g, x, stats)
+    _nhwc_check("adain_grad_stats", g, g, x)
+    B, H, W, C = g.shape
+    if tuple(stats.shape) != (B, C, 2) or not stats.is_contiguous():
+        raise _lib.VtError("adain_grad_stats: stats must be a contiguous [B, C, 2] table")
+    sums = torch.empty((B, C, 2), device=g.device, dtype=torch.float32)
+    check(_lib.load().vt_adain_grad_stats_nhwc(g.data_ptr(), x.data_ptr(), stats.data_ptr(), B, H * W, C, sums.data_ptr(),
+                                               _grad_ws(B, H * W, C, g.device).data_ptr(), _stream()))
+    return sums
+
+
+def act_grad(g: torch.Tensor, ref: Optional[torch.Tensor] = None, slope: float = 0.2, gain: float = 1.0,
+             res: Optional[torch.Tensor] = None, beta: float = 1.0, adain: Optional[Tuple] = None, bias_grad: bool = False):
+    """Backward of an activation (and optionally of the AdaIN in front of it) on NHWC tensors:
+    ``out = beta * res + gate(ref) * gain * T(g)``, gate(ref) = ref > 0 ? 1 : slope (``ref``: the LeakyReLU's own output),
+    T(g) = g, or with ``adain = (x, stats, gamma_beta, sums)`` the instance-norm + affine backward
+    ``gamma * rstd * ((g - m_g) - (x - mean) * rstd * m_gx)`` (``sums`` from :func:`adain_grad_stats`).
+    ``bias_grad``: also return the per-channel sum of ``out`` ([C]), reduced in the same pass."""
+    x, stats, gb, sums = adain if adain is not None else (None, None, None, None)
+    _req_cuda(g, ref, res, x, stats, gb, sums)
+    _nhwc_check("act_grad", g, g, ref, res, x)
+    B, H, W, C = g.shape
+    if adain is not None:
+        if tuple(stats.shape) != (B, C, 2) or tuple(sums.shape) != (B, C, 2) or tuple(gb.shape) != (B, 2 * C):
+            raise _lib.VtError("act_grad: AdaIN tables must be stats/sums [B, C, 2] and gamma_beta [B, 2C]")
+        stats, gb, sums = stats.contiguous(), gb.contiguous(), sums.contiguous()
+    out = torch.empty_like(g)
+    bg = torch.empty((C,), device=g.device, dtype=torch.float32) if bias_grad else None
+    ws = _grad_ws(B, H * W, C, g.device) if bias_grad else None
+    check(_lib.load().vt_act_grad_nhwc(g.data_ptr(), _ptr(ref), slope, gain, _ptr(res), beta, _ptr(x), _ptr(stats), _ptr(gb),
+                                       _ptr(sums), B, H * W, C, out.data_ptr(), _ptr(bg), _ptr(ws), _stream()))
+    return (out, bg) if bias_grad else out
+
+
 def affine_fold_weights(w: torch.Tensor, stats: torch.Tensor, gamma_beta: torch.Tensor):
     """Fold AdaIN's per-(b,c) affine into conv weights ``w`` [1, taps, N, C2] -> (w' [B, taps, N, C2], k [B, taps, N])."""
     _req_cuda(w, stats, gamma_beta)

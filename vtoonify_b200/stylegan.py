@@ -124,6 +124,7 @@ class EqualConv2d(nn.Module):
         self.dilation = dilation
         self.bias = nn.Parameter(torch.zeros(out_channel)) if bias else None
         self._w = _PreppedWeight()
+        self._wt = _PreppedWeight()          # transposed weight of the input gradient (encoder_grad)
 
     def forward_nhwc(self, x, **epi):
         return _conv_plain_nhwc(x, self.weight, self._w, self.scale, epi.pop("bias", self.bias), self.stride,

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 from torch import nn
 
-from . import ops
+from . import encoder_grad, ops
 from ._lib import ACT_LRELU, ACT_NONE, ACT_RELU_TANH
 from .dualstylegan import AdaptiveInstanceNorm, AdaResBlock, DualStyleGAN, Linear
 from .stylegan import Generator, _PreppedWeight
@@ -37,6 +37,7 @@ class Conv2d(nn.Module):
             self.bias = None
         self._w = _PreppedWeight()
         self._wp = _PreppedWeight()
+        self._wt = _PreppedWeight()          # transposed weight of the input gradient (encoder_grad)
 
     def forward_nhwc(self, x, act=ACT_NONE, slope=0.2, gain=1.0, res=None, alpha=1.0, beta=1.0, x2=None, x2_scale=None,
                      want_stats=False):
@@ -258,6 +259,8 @@ class VToonify(ops.WeightsEpochMixin, nn.Module):
     def _forward(self, x, style, d_s, return_mask, return_feat):
         D = self.backbone == 'dualstylegan'
         adastyles, resstyles = ops.style_cached(self, "styles", lambda: self._styles(style))
+        if return_feat and encoder_grad.takes_autograd(self, x):
+            return encoder_grad.feat_with_grad(self, x, style, d_s, resstyles)
 
         # encoder: downsampling conv blocks, then the res blocks (interleaved with dilated ModRes for D)
         feat = ops.to_nhwc(x, ops._pad32(x.shape[1]))

@@ -331,6 +331,15 @@ int vt_act_grad_nhwc(const float* g, const float* ref, float slope, float gain, 
                      const float* stats, const float* gamma_beta, const float* sums, int B, int64_t HW, int C, float* out,
                      float* bias_grad, void* ws, void* stream);
 
+/* ---- minibatch standard deviation of the StyleGAN discriminator (model/vtoonify.py:67-75), NHWC [B, HW, C] ------------------ */
+/* group = min(B, 4) in the reference; B % group != 0 is an error.  Sample b is in column b % (B / group); per column the statistic
+ * is the mean over (p, c) of sqrt(biased variance over the group + 1e-8).  Fixed-order double reductions, no atomics.
+ * Forward: out [B, HW, c_out] = x in channels [0, C), the column's statistic in channel C, zeros in (C, c_out); c_out > C. */
+int vt_mbstd_nhwc_f32(const float* x, float* out, int B, int group, int64_t HW, int C, int c_out, void* stream);
+/* Backward: gin [B, HW, c_in] is the gradient of the forward's out (the forward's x is re-read) -> gx [B, HW, C] = gin's first C
+ * channels plus the statistic's path, the column's sum of gin[..., C] times d(statistic)/dx. */
+int vt_mbstd_grad_nhwc_f32(const float* gin, const float* x, float* gx, int B, int group, int64_t HW, int C, int c_in, void* stream);
+
 /* ---- pSp encoder helpers (model/encoder/encoders/helpers.py:56-119, psp_encoders.py:72-88) ---------------- */
 /* out[b,y,x,c] = x[b,y,x,c] * gate[b,c] + sc[b, y*sc_stride, x*sc_stride, c]   (SE gate + shortcut add; gate may be NULL = 1,
  * sc: NHWC [B, Hs, Ws, C] with Hs >= (H-1)*sc_stride+1; MaxPool2d(1, stride) shortcut == strided sampling) */

@@ -753,3 +753,131 @@ extern "C" int vt_act_grad_nhwc(const float* g, const float* ref, float slope, f
   }
   return 0;
 }
+
+// ---- minibatch standard deviation of the StyleGAN discriminator (model/vtoonify.py:67-75) --------------------------------------
+// Sample b is in column m = b % M of its group (M = B / group, the reference's out.view(group, -1, ...)).  Per column the statistic
+// is mean over (h, w, c) of sqrt(var_g + 1e-8), var_g the biased variance over the group; every sample of the column gets it as
+// one more channel.  One block per column; every sum is in double and in a fixed order (thread-strided, then a shared-memory tree),
+// so reruns are bit-identical.
+namespace {
+
+constexpr int MBSTD_THREADS = 256;
+constexpr int MBSTD_MAX_GROUP = 4;
+
+__device__ double mbstd_block_sum(double v, double* sh) {
+  sh[threadIdx.x] = v;
+  __syncthreads();
+  for (int s = MBSTD_THREADS / 2; s > 0; s >>= 1) {
+    if (threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
+    __syncthreads();
+  }
+  const double r = sh[0];
+  __syncthreads();
+  return r;
+}
+
+// x [B, HW, C] -> out [B, HW, c_out]: channels [0, C) = x, channel C = the column's statistic, (C, c_out) = 0
+template <int G>
+__global__ void __launch_bounds__(MBSTD_THREADS)
+mbstd_kernel(const float* __restrict__ x, float* __restrict__ out, int M, int64_t HW, int C, int c_out, double inv_p) {
+  __shared__ double sh[MBSTD_THREADS];
+  const int m = blockIdx.x;
+  const int P = (int)HW * C;
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < P; i += MBSTD_THREADS) {
+    const int p = i / C, c = i % C;
+    double v[G], mean = 0.0;
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      const int64_t b = (int64_t)g * M + m;
+      v[g] = (double)__ldg(x + b * P + i);
+      out[(b * HW + p) * c_out + c] = (float)v[g];
+      mean += v[g];
+    }
+    mean *= 1.0 / G;
+    double var = 0.0;
+#pragma unroll
+    for (int g = 0; g < G; ++g) var += (v[g] - mean) * (v[g] - mean);
+    acc += (double)sqrtf((float)(var * (1.0 / G) + 1e-8));
+  }
+  const float s = (float)(mbstd_block_sum(acc, sh) * inv_p);
+  const int tail = c_out - C;
+  for (int i = threadIdx.x; i < G * (int)HW * tail; i += MBSTD_THREADS) {
+    const int g = i / ((int)HW * tail), p = (i / tail) % (int)HW, c = i % tail;
+    out[(((int64_t)g * M + m) * HW + p) * c_out + C + c] = c == 0 ? s : 0.f;
+  }
+}
+
+// gin [B, HW, c_in] (the gradient of mbstd_kernel's output) -> gx [B, HW, C] = gin[..., :C] + d(statistic)/dx * (sum over the
+// column's samples and pixels of gin[..., C]).  d sqrt(var + eps)/dx_g = (x_g - mean) / (G * sqrt(var + eps)).
+template <int G>
+__global__ void __launch_bounds__(MBSTD_THREADS)
+mbstd_grad_kernel(const float* __restrict__ gin, const float* __restrict__ x, float* __restrict__ gx, int M, int64_t HW, int C,
+                  int c_in, double inv_pg) {
+  __shared__ double sh[MBSTD_THREADS];
+  const int m = blockIdx.x;
+  const int P = (int)HW * C;
+  double part = 0.0;
+  for (int i = threadIdx.x; i < G * (int)HW; i += MBSTD_THREADS) {
+    const int64_t g = i / (int)HW, p = i % (int)HW;
+    part += (double)__ldg(gin + ((g * M + m) * HW + p) * c_in + C);
+  }
+  const double coef = mbstd_block_sum(part, sh) * inv_pg;
+  for (int i = threadIdx.x; i < P; i += MBSTD_THREADS) {
+    const int p = i / C, c = i % C;
+    double v[G], mean = 0.0;
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      v[g] = (double)__ldg(x + ((int64_t)g * M + m) * P + i);
+      mean += v[g];
+    }
+    mean *= 1.0 / G;
+    double var = 0.0;
+#pragma unroll
+    for (int g = 0; g < G; ++g) var += (v[g] - mean) * (v[g] - mean);
+    const double k = coef * (double)rsqrtf((float)(var * (1.0 / G) + 1e-8));
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      const int64_t b = (int64_t)g * M + m;
+      gx[b * P + i] = (float)((double)__ldg(gin + (b * HW + p) * c_in + c) + k * (v[g] - mean));
+    }
+  }
+}
+
+}  // namespace
+
+#define VT_MBSTD_CHECK(name, c_other)                                                                                  \
+  VT_CHECK(B >= 1 && group >= 1 && group <= MBSTD_MAX_GROUP && HW >= 1 && C >= 1 && c_other > C &&                   \
+           HW * c_other * MBSTD_MAX_GROUP < (1LL << 31), name ": bad shape (group 1..4, C < c_pad, small planes)");                                                                 \
+  VT_CHECK(B % group == 0, name ": batch %d is not a multiple of the group size %d", B, group)
+
+extern "C" int vt_mbstd_nhwc_f32(const float* x, float* out, int B, int group, int64_t HW, int C, int c_out, void* stream) {
+  VT_CHECK(x && out, "mbstd: null pointer");
+  VT_MBSTD_CHECK("mbstd", c_out);
+  const int M = B / group;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (group) {
+    case 1: mbstd_kernel<1><<<(unsigned)M, MBSTD_THREADS, 0, st>>>(x, out, M, HW, C, c_out, 1.0 / ((double)HW * C)); break;
+    case 2: mbstd_kernel<2><<<(unsigned)M, MBSTD_THREADS, 0, st>>>(x, out, M, HW, C, c_out, 1.0 / ((double)HW * C)); break;
+    case 3: mbstd_kernel<3><<<(unsigned)M, MBSTD_THREADS, 0, st>>>(x, out, M, HW, C, c_out, 1.0 / ((double)HW * C)); break;
+    default: mbstd_kernel<4><<<(unsigned)M, MBSTD_THREADS, 0, st>>>(x, out, M, HW, C, c_out, 1.0 / ((double)HW * C)); break;
+  }
+  VT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int vt_mbstd_grad_nhwc_f32(const float* gin, const float* x, float* gx, int B, int group, int64_t HW, int C, int c_in,
+                                      void* stream) {
+  VT_CHECK(gin && x && gx, "mbstd_grad: null pointer");
+  VT_MBSTD_CHECK("mbstd_grad", c_in);
+  const int M = B / group;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (group) {
+    case 1: mbstd_grad_kernel<1><<<(unsigned)M, MBSTD_THREADS, 0, st>>>(gin, x, gx, M, HW, C, c_in, 1.0 / ((double)HW * C * group)); break;
+    case 2: mbstd_grad_kernel<2><<<(unsigned)M, MBSTD_THREADS, 0, st>>>(gin, x, gx, M, HW, C, c_in, 1.0 / ((double)HW * C * group)); break;
+    case 3: mbstd_grad_kernel<3><<<(unsigned)M, MBSTD_THREADS, 0, st>>>(gin, x, gx, M, HW, C, c_in, 1.0 / ((double)HW * C * group)); break;
+    default: mbstd_grad_kernel<4><<<(unsigned)M, MBSTD_THREADS, 0, st>>>(gin, x, gx, M, HW, C, c_in, 1.0 / ((double)HW * C * group)); break;
+  }
+  VT_LAUNCH_CHECK();
+  return 0;
+}

@@ -876,6 +876,33 @@ def act_grad(g: torch.Tensor, ref: Optional[torch.Tensor] = None, slope: float =
     return (out, bg) if bias_grad else out
 
 
+def mbstd(x: torch.Tensor, group: int) -> torch.Tensor:
+    """Minibatch standard deviation of the StyleGAN discriminator (model/vtoonify.py:67-75) on NHWC ``x`` [B, H, W, C]:
+    ``[B, H, W, pad32(C + 1)]`` holding x, then the statistic of the sample's column ``b % (B / group)``, then zeros."""
+    _req_cuda(x)
+    B, H, W, C = x.shape
+    if B % group:
+        raise _lib.VtError(f"mbstd: batch {B} is not a multiple of the group size {group}")
+    x = x.contiguous()
+    out = torch.empty((B, H, W, _pad32(C + 1)), device=x.device, dtype=torch.float32)
+    check(_lib.load().vt_mbstd_nhwc_f32(x.data_ptr(), out.data_ptr(), B, group, H * W, C, out.shape[3], _stream()))
+    return out
+
+
+def mbstd_grad(g: torch.Tensor, x: torch.Tensor, group: int) -> torch.Tensor:
+    """Backward of :func:`mbstd`: ``g`` [B, H, W, c_pad] (gradient of its output), ``x`` its input -> gradient of ``x``."""
+    _req_cuda(g, x)
+    B, H, W, C = x.shape
+    if B % group:
+        raise _lib.VtError(f"mbstd_grad: batch {B} is not a multiple of the group size {group}")
+    if g.shape[:3] != x.shape[:3]:
+        raise _lib.VtError("mbstd_grad: g and x must have the same batch and map size")
+    g, x = g.contiguous(), x.contiguous()
+    out = torch.empty_like(x)
+    check(_lib.load().vt_mbstd_grad_nhwc_f32(g.data_ptr(), x.data_ptr(), out.data_ptr(), B, group, H * W, C, g.shape[3], _stream()))
+    return out
+
+
 def affine_fold_weights(w: torch.Tensor, stats: torch.Tensor, gamma_beta: torch.Tensor):
     """Fold AdaIN's per-(b,c) affine into conv weights ``w`` [1, taps, N, C2] -> (w' [B, taps, N, C2], k [B, taps, N])."""
     _req_cuda(w, stats, gamma_beta)

@@ -9,7 +9,8 @@ Differences in *how* (not what):
     implicit GEMM over the batch (per-sample weight tile selected by the TMA coordinate);
   * ``StyledConv`` fuses noise + bias + leaky-relu into the conv epilogue (or into the FIR pass after the
     transposed conv); ``ToRGB`` fuses the 1x1 modulated conv, bias, skip ``Upsample`` and add in one kernel.
-Forward-only (inference), CUDA only.
+Forward-only (inference), CUDA only; the discriminator's ResBlock / ConvLayer(downsample=True) have gradients through
+vtoonify_b200.discriminator.
 """
 import math
 import random
@@ -20,6 +21,8 @@ from torch import nn
 from . import ops
 from .op import FusedLeakyReLU, fused_leaky_relu, upfirdn2d, conv2d_gradfix  # noqa: F401
 from ._lib import ACT_LRELU, ACT_NONE
+
+_R2 = 1.0 / math.sqrt(2.0)
 
 
 class PixelNorm(nn.Module):
@@ -500,15 +503,69 @@ class ConvLayer(nn.Sequential):
             layers.append(FusedLeakyReLU(out_channel, bias=bias))
         super().__init__(*layers)
 
-    def forward_nhwc(self, x, res=None, alpha=1.0, beta=1.0, src_affine=None, want_stats=False):
-        """Fused conv + FusedLeakyReLU (+ ``v*alpha + beta*res``) for the non-downsampling form; ``src_affine``: AdaIN table
-        applied to the input inside the convolution; ``want_stats``: ``(out, instance-norm statistics of out)``."""
+    def forward_nhwc(self, x, res=None, alpha=1.0, beta=1.0, src_affine=None, want_stats=False, blurred=None):
+        """Fused conv + FusedLeakyReLU (+ ``v*alpha + beta*res``); ``src_affine``: AdaIN table applied to the input inside the
+        convolution; ``want_stats``: ``(out, instance-norm statistics of out)`` (non-downsampling form).
+
+        The downsampling form (discriminator) is a stride-2 convolution on ``blurred`` = ``blur_pad2(x)`` (computed here when not
+        given): the 4x4 Blur with pad (2, 2), ``[B, H+1, W+1, C]``.  The reference's blur pad (p0, p1) with p0 <= 2 reads that tensor
+        shifted by 2 - p0 (the 1x1 skip's pad (1, 1) blur is its tap (1, 1)), so one blur serves every downsampling layer on x."""
         mods = list(self)
         if isinstance(mods[0], Blur):
-            raise NotImplementedError("ConvLayer(downsample=True) is discriminator-only (training)")
+            if src_affine is not None or want_stats:
+                raise NotImplementedError("ConvLayer(downsample=True): no src_affine / want_stats")
+            conv = mods[1]
+            k, (p0, p1) = conv.weight.shape[2], mods[0].pad
+            if tuple(mods[0].kernel.shape) != (4, 4) or p0 > 2:
+                raise NotImplementedError("ConvLayer(downsample=True) supports the 4-tap blur kernel")
+            xb = blur_pad2(x, mods[0].kernel) if blurred is None else blurred
+            B, H, W, _ = x.shape
+            Ho = (H + p0 + p1 - 3 - k) // 2 + 1
+            Wo = (W + p0 + p1 - 3 - k) // 2 + 1
+            off = 2 - p0
+            taps = [(ky + off, kx + off, ky * k + kx) for ky in range(k) for kx in range(k)]
+            w = conv._w.get(conv.weight, conv.scale, xb.shape[3])
+            epi = dict(act=ACT_LRELU, bias=mods[2].bias, slope=mods[2].negative_slope, gain=mods[2].scale) if len(mods) > 2 else {}
+            return ops.conv2d_nhwc([xb], w, taps, 2, Ho, Wo, res=res, alpha=alpha, beta=beta, **epi)
         conv = mods[0]
         if len(mods) > 1:
             act = mods[1]
             return conv.forward_nhwc(x, bias=act.bias, act=ACT_LRELU, slope=act.negative_slope, gain=act.scale,
                                      res=res, alpha=alpha, beta=beta, src_affine=src_affine, want_stats=want_stats)
         return conv.forward_nhwc(x, res=res, alpha=alpha, beta=beta, src_affine=src_affine, want_stats=want_stats)
+
+
+def blur_pad2(x, kernel):
+    """``Blur(kernel, pad=(2, 2))`` of NHWC ``x``: ``[B, H+1, W+1, C]``, the input of every downsampling ConvLayer."""
+    return ops.fir_nhwc(x, kernel, (2, 2))
+
+
+class ResBlock(nn.Module):
+    """model/stylegan/model.py:640-658: ``(conv2(conv1(x)) + skip(x)) / sqrt(2)``, both halves downsampling by 2.
+
+    NHWC: conv1 with bias + FusedLeakyReLU in its epilogue; conv2 (3x3, stride 2) on the pad (2, 2) blur of conv1's output with its
+    bias + FusedLeakyReLU; the skip (1x1, stride 2, tap (1, 1)) on the pad (2, 2) blur of x, whose epilogue adds conv2's output:
+    ``(a2 + skip) / sqrt(2)`` with ``alpha = beta = 1/sqrt(2)``, so the block output costs no extra pass and ``a2`` (the gate's
+    reference in the backward) is kept."""
+
+    def __init__(self, in_channel, out_channel, blur_kernel=[1, 3, 3, 1]):
+        super().__init__()
+        self.conv1 = ConvLayer(in_channel, in_channel, 3)
+        self.conv2 = ConvLayer(in_channel, out_channel, 3, downsample=True, blur_kernel=blur_kernel)
+        self.skip = ConvLayer(in_channel, out_channel, 1, downsample=True, activate=False, bias=False, blur_kernel=blur_kernel)
+
+    def forward_nhwc(self, x, rec=None):
+        """NHWC ``x`` -> NHWC block output; ``rec`` (a list): appends what the backward reads."""
+        a1 = self.conv1.forward_nhwc(x)
+        a1b = blur_pad2(a1, self.conv2[0].kernel)
+        a2 = self.conv2.forward_nhwc(a1, blurred=a1b)
+        xb = blur_pad2(x, self.skip[0].kernel)
+        out = self.skip.forward_nhwc(x, blurred=xb, res=a2, alpha=_R2, beta=_R2)
+        if rec is not None:
+            rec.append((self, x, a1, a1b, a2, xb))
+        return out
+
+    def forward(self, input):
+        C = input.shape[1]
+        x = ops.to_nhwc(input, ops._pad32(C) if C % 32 else None)
+        return ops.nhwc_as_nchw_view(self.forward_nhwc(x))

@@ -16,10 +16,57 @@ import numpy as np
 import torch
 from torch import nn
 
-from . import encoder_grad, ops
+from . import discriminator, encoder_grad, ops
 from ._lib import ACT_LRELU, ACT_NONE, ACT_RELU_TANH
 from .dualstylegan import AdaptiveInstanceNorm, AdaResBlock, DualStyleGAN, Linear
-from .stylegan import Generator, _PreppedWeight
+from .stylegan import ConvLayer, EqualLinear, Generator, ResBlock, _PreppedWeight
+
+
+class ConditionalDiscriminator(nn.Module):
+    """model/vtoonify.py:10-89 — same constructor, ``forward(input, degree_label=None, style_ind=None)``, return value and
+    state_dict keys.  The convolutional trunk, the minibatch standard deviation and ``final_linear`` run NHWC on the library's
+    kernels, with gradients into ``input`` and every parameter of ``convs``, ``final_conv`` and ``final_linear``
+    (vtoonify_b200.discriminator); ``label_mapper``, ``style_mapper`` and the conditioning product are ordinary torch modules."""
+
+    def __init__(self, size, channel_multiplier=2, blur_kernel=[1, 3, 3, 1], use_condition=False, style_num=None):
+        super().__init__()
+        channels = {4: 512, 8: 512, 16: 512, 32: 512, 64: 256 * channel_multiplier, 128: 128 * channel_multiplier,
+                    256: 64 * channel_multiplier, 512: 32 * channel_multiplier, 1024: 16 * channel_multiplier}
+        convs = [ConvLayer(3, channels[size], 1)]
+        log_size = int(math.log(size, 2))
+        in_channel = channels[size]
+        for i in range(log_size, 2, -1):
+            out_channel = channels[2 ** (i - 1)]
+            convs.append(ResBlock(in_channel, out_channel, blur_kernel))
+            in_channel = out_channel
+        self.convs = nn.Sequential(*convs)
+        self.stddev_group = 4
+        self.stddev_feat = 1
+        self.use_condition = use_condition
+        if self.use_condition:
+            self.condition_dim = 128
+            self.label_mapper = nn.Sequential(
+                nn.Linear(1, 64),
+                nn.LeakyReLU(negative_slope=0.2, inplace=True),
+                nn.Linear(64, 64),
+                nn.LeakyReLU(negative_slope=0.2, inplace=True),
+                nn.Linear(64, self.condition_dim // 2),
+            )
+            self.style_mapper = nn.Embedding(style_num, self.condition_dim - self.condition_dim // 2)
+        else:
+            self.condition_dim = 1
+        self.final_conv = ConvLayer(in_channel + 1, channels[4], 3)
+        self.final_linear = nn.Sequential(
+            EqualLinear(channels[4] * 4 * 4, channels[4], activation="fused_lrelu"),
+            EqualLinear(channels[4], self.condition_dim),
+        )
+
+    def forward(self, input, degree_label=None, style_ind=None):
+        h = discriminator.final_linear_out(self, input)
+        if self.use_condition:
+            condition = torch.cat((self.label_mapper(degree_label), self.style_mapper(style_ind)), dim=1)
+            return (h * condition).sum(dim=1, keepdim=True) * (1 / np.sqrt(self.condition_dim))
+        return h
 
 
 class Conv2d(nn.Module):

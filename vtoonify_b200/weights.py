@@ -10,6 +10,10 @@ import zlib
 import torch
 
 
+# top-level keys of a ConditionalDiscriminator state_dict that hold an EqualConv2d / EqualLinear weight (no other model's keys match)
+DISCRIMINATOR_EQUAL_WEIGHT = re.compile(r"^(convs\.\d+\.(0|conv1\.0|conv2\.1|skip\.1)|final_conv\.0|final_linear\.\d)\.weight$")
+
+
 def det_tensor(key: str, ref: torch.Tensor, seed: int = 0) -> torch.Tensor:
     shape = tuple(ref.shape)
     g = torch.Generator(device="cpu")
@@ -33,8 +37,12 @@ def det_tensor(key: str, ref: torch.Tensor, seed: int = 0) -> torch.Tensor:
         return 1.0 + 0.1 * r                                    # BatchNorm gamma
     if ref.dim() == 1 and re.search(r"(input_layer\.2|res_layer\.2)\.weight$", key):
         return 0.25 + 0.05 * r                                   # PReLU slopes
-    if key.endswith("blur.kernel") or key.endswith("upsample.kernel"):
+    if key.endswith("blur.kernel") or key.endswith("upsample.kernel") or key.endswith(".0.kernel"):
         return ref.detach().clone().float()                      # FIR taps are architecture constants
+    if DISCRIMINATOR_EQUAL_WEIGHT.search(key):
+        return r                                                 # ConditionalDiscriminator's EqualConv2d / EqualLinear weights:
+                                                                 # randn, as the reference initialises them (the layer's own
+                                                                 # 1/sqrt(fan_in) keeps activations O(1))
     if "noises.noise_" in key or key.endswith("input.input"):
         return r
     if key.endswith("modulation.weight"):

@@ -237,8 +237,9 @@ extern "C" int vt_nhwc_to_nchw_f32(const float* in, float* out, int B, int C, in
 
 extern "C" int vt_axpby_f32(const float* a, const float* b, float* out, int64_t n, float scale_a, float scale_b,
                             int round_tf32, void* stream) {
-  VT_CHECK(a && out && n >= 0, "axpby: bad args");
-  if (n == 0) return 0;
+  VT_CHECK(n >= 0, "axpby: negative size");
+  if (n == 0) return 0;                 // empty tensors may have null data pointers
+  VT_CHECK(a && out, "axpby: null pointer");
   axpby_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(a, b, out, n, scale_a, scale_b, round_tf32);
   VT_LAUNCH_CHECK();
   return 0;

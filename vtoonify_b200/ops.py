@@ -333,7 +333,12 @@ def channel_sum(x: torch.Tensor) -> torch.Tensor:
 # ----------------------------------------------------------------------------------------------
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], w_scale: float = 1.0,
            b_scale: float = 1.0, act: int = 0) -> torch.Tensor:
-    """``act``: 0 none, 1 fused_leaky_relu (0.2, *sqrt2), 2 LeakyReLU(0.2)."""
+    """``act``: 0 none, 1 fused_leaky_relu (0.2, *sqrt2), 2 LeakyReLU(0.2), 3 ReLU, 4 sigmoid."""
+    if weight.dim() != 2 or x.dim() < 1 or weight.shape[1] != x.shape[-1]:
+        raise _lib.VtError(f"linear: weight {tuple(weight.shape)} does not match input {tuple(x.shape)}: "
+                           "it must be [out_dim, in_dim] with in_dim the last dim of the input")
+    if bias is not None and bias.numel() != weight.shape[0]:
+        raise _lib.VtError(f"linear: bias has {bias.numel()} elements, out_dim is {weight.shape[0]}")
     _req_cuda(x, weight, bias)
     shp = x.shape
     x2 = x.reshape(-1, shp[-1]).contiguous()
@@ -362,6 +367,10 @@ def prep_weights(W: torch.Tensor, style: Optional[torch.Tensor] = None, scale: f
                  cin_pad: Optional[int] = None, round_tf32: Optional[bool] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``W`` [Cout,Cin,kh,kw] (+ optional per-sample ``style`` [B,Cin]) -> conv-kernel layout
     ``[wB, kh*kw, Cout, cin_pad]`` = (scale*W)*style*demod (model/stylegan/model.py:259-267)."""
+    if W.dim() != 4:
+        raise _lib.VtError(f"prep_weights: W must be [Cout, Cin, kh, kw] (got {tuple(W.shape)})")
+    if style is not None and (style.dim() != 2 or style.shape[1] != W.shape[1]):
+        raise _lib.VtError(f"prep_weights: style {tuple(style.shape)} must be [wB, Cin] with Cin = {W.shape[1]}")
     _req_cuda(W, style)
     Cout, Cin, kh, kw = W.shape
     cin_pad = _pad32(Cin) if cin_pad is None else cin_pad
@@ -917,8 +926,14 @@ def affine_fold_weights(w: torch.Tensor, stats: torch.Tensor, gamma_beta: torch.
 
 def gate_shortcut_add(x: torch.Tensor, gate: Optional[torch.Tensor], sc: torch.Tensor, sc_stride: int = 1) -> torch.Tensor:
     """``x * gate[b,c] + sc[b, y*s, x*s, c]`` (SE gate and residual shortcut; a MaxPool2d(1, s) shortcut is the strided read)."""
-    _req_cuda(x, gate, sc)
+    if x.dim() != 4 or sc.dim() != 4 or not x.is_contiguous() or not sc.is_contiguous():
+        raise _lib.VtError(f"gate_shortcut_add: x {tuple(x.shape)} and sc {tuple(sc.shape)} must be contiguous NHWC tensors")
     B, H, W, C = x.shape
+    if sc.shape[0] != B or sc.shape[3] != C:
+        raise _lib.VtError(f"gate_shortcut_add: sc {tuple(sc.shape)} does not match the batch and channels of x {tuple(x.shape)}")
+    if gate is not None and (gate.shape[0] != B or gate.numel() != B * C):
+        raise _lib.VtError(f"gate_shortcut_add: gate {tuple(gate.shape)} must hold [B, C] = [{B}, {C}] values")
+    _req_cuda(x, gate, sc)
     out = torch.empty_like(x)
     check(_lib.load().vt_gate_shortcut_add_nhwc(x.data_ptr(), _ptr(None if gate is None else gate.contiguous()), sc.data_ptr(),
                                                 out.data_ptr(), B, H, W, C, sc.shape[1], sc.shape[2], sc_stride, _round_flag(), _stream()))
@@ -927,6 +942,10 @@ def gate_shortcut_add(x: torch.Tensor, gate: Optional[torch.Tensor], sc: torch.T
 
 def bilinear_add(x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
     """``F.interpolate(x, size=y.shape[1:3], mode='bilinear', align_corners=True) + y`` on NHWC tensors."""
+    if x.dim() != 4 or y.dim() != 4 or not x.is_contiguous() or not y.is_contiguous():
+        raise _lib.VtError(f"bilinear_add: x {tuple(x.shape)} and y {tuple(y.shape)} must be contiguous NHWC tensors")
+    if x.shape[0] != y.shape[0] or x.shape[3] != y.shape[3]:
+        raise _lib.VtError(f"bilinear_add: x {tuple(x.shape)} and y {tuple(y.shape)} differ in batch or channels")
     _req_cuda(x, y)
     B, h, w, C = x.shape
     _, H, W, _ = y.shape
@@ -937,6 +956,9 @@ def bilinear_add(x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
 
 def axpby(a: torch.Tensor, b: Optional[torch.Tensor], sa: float, sb: float = 0.0, round_tf32: Optional[bool] = None,
           out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``out = a * sa + b * sb`` elementwise over ``a.numel()`` elements (``b`` None: ``a * sa``)."""
+    if b is not None and b.numel() != a.numel():
+        raise _lib.VtError(f"axpby: b has {b.numel()} elements, a has {a.numel()}")
     _req_cuda(a, b, out)
     if not a.is_contiguous() or (b is not None and not b.is_contiguous()):
         a, b = a.contiguous(), (None if b is None else b.contiguous())

@@ -26,10 +26,13 @@ _R2 = 1.0 / math.sqrt(2.0)
 
 
 class PixelNorm(nn.Module):
-    """model/stylegan/model.py:13-18"""
+    """model/stylegan/model.py:13-18: normalises over dim 1, for any rank >= 2 (the kernel normalises the last dim, so dim 1
+    is moved last and back)."""
 
     def forward(self, input):
-        return ops.pixelnorm(input)
+        if input.dim() <= 2:
+            return ops.pixelnorm(input)
+        return ops.pixelnorm(input.movedim(1, -1)).movedim(-1, 1)
 
 
 def make_kernel(k):

@@ -326,10 +326,34 @@ int vt_adain_grad_stats_nhwc(const float* g, const float* x, const float* stats,
 /* Elementwise half: out = beta * res + gate(ref) * gain * T(g), gate(ref) = ref > 0 ? 1 : slope (ref NULL: 1), res may be NULL.
  * T(g) = g when x is NULL; otherwise the AdaIN backward gamma * rstd * ((g - m_g) - (x - mean) * rstd * m_gx) with
  * m_g, m_gx = sums / HW from vt_adain_grad_stats_nhwc and gamma from gamma_beta [B][2C] (gamma then beta).
- * bias_grad (may be NULL): [C] = sum over b and p of out, from per-chunk partials of the same pass. */
+ * bias_grad (may be NULL): [C] = sum over b and p of out, from per-chunk partials of the same pass.  With bias_grad, out may be
+ * NULL: only the sums are produced (ops.channel_sum_nhwc). */
 int vt_act_grad_nhwc(const float* g, const float* ref, float slope, float gain, const float* res, float beta, const float* x,
                      const float* stats, const float* gamma_beta, const float* sums, int B, int64_t HW, int C, float* out,
                      float* bias_grad, void* ws, void* stream);
+
+/* ---- backward of the generator tail of VToonify.forward (G step), NHWC [B, HW, C], 16-byte aligned tensors ----------------- */
+/* StyledConv gate with the ToRGB adjoint: out = gate(ref) * gain * (g + sum_k w_rgb[b][k][c] * g_rgb[b][k][p]); g may be NULL (0),
+ * g_rgb planar [B][3][HW] (the image gradient, read directly), w_rgb [wB][3][w_cstride] (wB 1 or B), gate(ref) = ref > 0 ? 1 : slope. */
+int vt_torgb_gate_grad_nhwc(const float* g, const float* g_rgb, const float* w_rgb, int wB, int w_cstride, const float* ref,
+                            float slope, float gain, int B, int64_t HW, int C, float* out, void* stream);
+/* bytes of the ws of vt_fusion_mask_grad_nhwc */
+int64_t vt_fusion_mask_grad_ws_bytes(int B, int64_t HW);
+/* Fusion mask head m = tanh(relu z): g_z[b][p] = (sum_c g_p * f_e + g_m[b][p]) * (1 - m^2) * [m > 0] (g_m planar, may be NULL), and
+ * bias_grad[0] = sum of g_z.  g_p: gradient of f_E * m.  Fixed-order double reductions. */
+int vt_fusion_mask_grad_nhwc(const float* g_p, const float* f_e, const float* m, const float* g_m, int B, int64_t HW, int C,
+                             float* g_z, float* bias_grad, void* ws, void* stream);
+/* AdaIN-backward sums of the mask head over the virtual concat A = cat(f_G, |f_G - f_E|) (2C channels, C <= 512): with
+ * u = conv2's input gradient, u[p][c'] = sum_t w2[t][c'] * g_z[p - (t / 3 - 1, t % 3 - 1)], sums[b][c'] = (sum_p u, sum_p u * ahat),
+ * ahat = (A - mean) * rstd, stats [B][2C][2].  w2 [9][2C] is conv2's weight tap-major.  u is never written.
+ * ws: vt_act_grad_ws_bytes(B, H * W, 2C) bytes. */
+int vt_fusion_adain_grad_stats_nhwc(const float* g_z, const float* w2, const float* f_g, const float* f_e, const float* stats,
+                                    int B, int H, int W, int C, float* sums, void* ws, void* stream);
+/* Elementwise pass of the mask head: T = the AdaIN backward of u (as vt_act_grad_nhwc with gamma_beta [B][4C]), s = sign(f_G - f_E)
+ * (sign(0) = 0): g_fg = g_dir + T[c] + s * T[C + c], g_fe = g_p * m - s * T[C + c] (g_dir may be NULL). */
+int vt_fusion_input_grad_nhwc(const float* g_z, const float* w2, const float* f_g, const float* f_e, const float* stats,
+                              const float* gamma_beta, const float* sums, const float* g_dir, const float* g_p, const float* m,
+                              int B, int H, int W, int C, float* g_fg, float* g_fe, void* stream);
 
 /* ---- minibatch standard deviation of the StyleGAN discriminator (model/vtoonify.py:67-75), NHWC [B, HW, C] ------------------ */
 /* group = min(B, 4) in the reference; B % group != 0 is an error.  Sample b is in column b % (B / group); per column the statistic

@@ -115,6 +115,11 @@ SYMBOLS = {
     "vt_act_grad_ws_bytes": (c_int64, [c_int, c_int64, c_int]),
     "vt_adain_grad_stats_nhwc": (c_int, [_P, _P, _P, c_int, c_int64, c_int, _P, _P, _P]),
     "vt_act_grad_nhwc": (c_int, [_P, _P, c_float, c_float, _P, c_float, _P, _P, _P, _P, c_int, c_int64, c_int, _P, _P, _P, _P]),
+    "vt_torgb_gate_grad_nhwc": (c_int, [_P, _P, _P, c_int, c_int, _P, c_float, c_float, c_int, c_int64, c_int, _P, _P]),
+    "vt_fusion_mask_grad_ws_bytes": (c_int64, [c_int, c_int64]),
+    "vt_fusion_mask_grad_nhwc": (c_int, [_P, _P, _P, _P, c_int, c_int64, c_int, _P, _P, _P, _P]),
+    "vt_fusion_adain_grad_stats_nhwc": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),
+    "vt_fusion_input_grad_nhwc": (c_int, [_P] * 10 + [c_int, c_int, c_int, c_int, _P, _P, _P]),
     "vt_mbstd_nhwc_f32": (c_int, [_P, _P, c_int, c_int, c_int64, c_int, c_int, _P]),
     "vt_mbstd_grad_nhwc_f32": (c_int, [_P, _P, _P, c_int, c_int, c_int64, c_int, c_int, _P]),
     "vt_gate_shortcut_add_nhwc": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),

@@ -653,7 +653,7 @@ act_grad_kernel(const float* __restrict__ g, const float* __restrict__ ref, floa
 #pragma unroll
         for (int i = 0; i < 4; ++i) t[i] = fmaf(beta, sa[i], t[i]);
       }
-      *reinterpret_cast<float4*>(out + o) = make_float4(t[0], t[1], t[2], t[3]);
+      if (out) *reinterpret_cast<float4*>(out + o) = make_float4(t[0], t[1], t[2], t[3]);
       if (ws) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) bs[i] += (double)t[i];
@@ -724,11 +724,11 @@ extern "C" int vt_adain_grad_stats_nhwc(const float* g, const float* x, const fl
 extern "C" int vt_act_grad_nhwc(const float* g, const float* ref, float slope, float gain, const float* res, float beta,
                                 const float* x, const float* stats, const float* gamma_beta, const float* sums, int B, int64_t HW,
                                 int C, float* out, float* bias_grad, void* ws, void* stream) {
-  VT_CHECK(g && out, "act_grad: null pointer");
+  VT_CHECK(g && (out || bias_grad), "act_grad: null pointer (out may be NULL only with bias_grad)");
   const bool adain = x != nullptr;
   VT_CHECK(!adain || (stats && gamma_beta && sums), "act_grad: the AdaIN form needs x, stats, gamma_beta and sums");
   VT_CHECK(!bias_grad || ws, "act_grad: bias_grad needs ws");
-  VT_CHECK(aligned16(g) && aligned16(out) && (!ref || aligned16(ref)) && (!res || aligned16(res)) && (!x || aligned16(x)) &&
+  VT_CHECK(aligned16(g) && (!out || aligned16(out)) && (!ref || aligned16(ref)) && (!res || aligned16(res)) && (!x || aligned16(x)) &&
            (!ws || aligned16(ws)), "act_grad: tensors must be 16-byte aligned");
   VT_GRAD_SHAPE_CHECK("act_grad");
   int64_t chunk, chunks;
@@ -751,6 +751,317 @@ extern "C" int vt_act_grad_nhwc(const float* g, const float* ref, float slope, f
     partials_sum_kernel<<<(unsigned)vt_cdiv(C, 8), 256, 0, st>>>(part, chunks * B, C, 1.f, bias_grad);
     VT_LAUNCH_CHECK();
   }
+  return 0;
+}
+
+// ---- backward of the generator tail of VToonify.forward (the G step of both training scripts) -----------------------------------
+//   vt_torgb_gate_grad_nhwc         : StyledConv gate with the ToRGB adjoint folded in, out = gate(ref) * gain * (g + w_rgb^T g_rgb)
+//   vt_fusion_mask_grad_nhwc        : g_z of the mask head m = tanh(relu z), and conv2's bias gradient
+//   vt_fusion_adain_grad_stats_nhwc : the AdaIN-backward sums over cat(f_G, |f_G - f_E|), the 2C-channel gradient recomputed per pixel
+//                                     from g_z (conv2's transposed 3x3) instead of being written
+//   vt_fusion_input_grad_nhwc       : g_{f_G} and g_{f_E} from the AdaIN backward, the |.| split and the f_E * m product
+// The reductions follow act_grad's scheme: per-block double partials, then a warp per entry adds them in a fixed order.
+namespace {
+
+constexpr int MASK_CHUNK = 256;      // pixels per block of the mask-gradient pass
+
+__global__ void __launch_bounds__(256)
+torgb_gate_grad_kernel(const float* __restrict__ g, const float* __restrict__ grgb, const float* __restrict__ w, int wB,
+                       int w_cstride, const float* __restrict__ ref, float slope, float gain, int B, int64_t HW, int C,
+                       float* __restrict__ out) {
+  const int nvec = C / 4;
+  const int64_t total = (int64_t)B * HW * nvec;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int v = (int)(i % nvec);
+    const int64_t bp = i / nvec;
+    const int b = (int)(bp / HW);
+    const int64_t p = bp - (int64_t)b * HW;
+    const float* gr = grgb + (int64_t)b * 3 * HW + p;
+    const float r0 = __ldg(gr), r1 = __ldg(gr + HW), r2 = __ldg(gr + 2 * HW);
+    const float* wp = w + (int64_t)(wB == 1 ? 0 : b) * 3 * w_cstride + v * 4;
+    const float4 w0 = __ldg(reinterpret_cast<const float4*>(wp));
+    const float4 w1 = __ldg(reinterpret_cast<const float4*>(wp + w_cstride));
+    const float4 w2 = __ldg(reinterpret_cast<const float4*>(wp + 2 * w_cstride));
+    float t[4] = {0.f, 0.f, 0.f, 0.f};
+    if (g) {
+      const float4 gv = __ldg(reinterpret_cast<const float4*>(g + bp * C + v * 4));
+      t[0] = gv.x; t[1] = gv.y; t[2] = gv.z; t[3] = gv.w;
+    }
+    t[0] = fmaf(w2.x, r2, fmaf(w1.x, r1, fmaf(w0.x, r0, t[0])));
+    t[1] = fmaf(w2.y, r2, fmaf(w1.y, r1, fmaf(w0.y, r0, t[1])));
+    t[2] = fmaf(w2.z, r2, fmaf(w1.z, r1, fmaf(w0.z, r0, t[2])));
+    t[3] = fmaf(w2.w, r2, fmaf(w1.w, r1, fmaf(w0.w, r0, t[3])));
+    const float4 rv = __ldg(reinterpret_cast<const float4*>(ref + bp * C + v * 4));
+    const float ra[4] = {rv.x, rv.y, rv.z, rv.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) t[k] = (ra[k] > 0.f ? t[k] : t[k] * slope) * gain;
+    *reinterpret_cast<float4*>(out + bp * C + v * 4) = make_float4(t[0], t[1], t[2], t[3]);
+  }
+}
+
+// One warp per pixel: s = sum_c g_p * f_e (double, lane-strided then a fixed shuffle tree); g_z = (s + g_m) * (1 - m^2) * [m > 0].
+// Per (chunk, b) the double sum of g_z over the chunk's pixels, warps added in a fixed order.
+__global__ void __launch_bounds__(256)
+fusion_mask_grad_kernel(const float* __restrict__ gp, const float* __restrict__ fe, const float* __restrict__ m,
+                        const float* __restrict__ gm, int64_t HW, int C, float* __restrict__ gz, double* __restrict__ ws) {
+  __shared__ double sw[8];
+  const int b = blockIdx.y, warp = threadIdx.x / 32, lane = threadIdx.x % 32, nvec = C / 4;
+  const int64_t p_begin = (int64_t)blockIdx.x * MASK_CHUNK;
+  const int64_t p_end = (p_begin + MASK_CHUNK < HW) ? p_begin + MASK_CHUNK : HW;
+  double acc = 0.0;
+  for (int64_t p = p_begin + warp; p < p_end; p += 8) {
+    const int64_t o = ((int64_t)b * HW + p) * C;
+    double s = 0.0;
+    for (int v = lane; v < nvec; v += 32) {
+      const float4 a = __ldg(reinterpret_cast<const float4*>(gp + o + v * 4));
+      const float4 e = __ldg(reinterpret_cast<const float4*>(fe + o + v * 4));
+      s = fma((double)a.x, (double)e.x, s);
+      s = fma((double)a.y, (double)e.y, s);
+      s = fma((double)a.z, (double)e.z, s);
+      s = fma((double)a.w, (double)e.w, s);
+    }
+#pragma unroll
+    for (int k = 16; k > 0; k >>= 1) s += __shfl_xor_sync(0xffffffffu, s, k);
+    const int64_t q = (int64_t)b * HW + p;
+    const float mv = m[q];
+    const float sg = (float)s + (gm ? gm[q] : 0.f);
+    const float z = mv > 0.f ? sg * (1.f - mv * mv) : 0.f;
+    if (lane == 0) gz[q] = z;
+    acc += (double)z;
+  }
+  if (lane == 0) sw[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int k = 0; k < 8; ++k) t += sw[k];
+    ws[(int64_t)blockIdx.x * gridDim.y + b] = t;
+  }
+}
+
+// the 9 values g_z[p - (ky - 1, kx - 1)] that conv2's transposed 3x3 reads at pixel (y, x), 0 outside the map
+__device__ __forceinline__ void fusion_taps(const float* __restrict__ gzb, int y, int x, int H, int W, float (&gt)[9]) {
+#pragma unroll
+  for (int t = 0; t < 9; ++t) {
+    const int yy = y - (t / 3 - 1), xx = x - (t % 3 - 1);
+    gt[t] = (yy < 0 || yy >= H || xx < 0 || xx >= W) ? 0.f : __ldg(gzb + (int64_t)yy * W + xx);
+  }
+}
+
+// u[c'] = sum over the taps of w2[t][c'] * gt[t]: the gradient at conv2's input, channels c' of the virtual concat
+// cat(f_G, |f_G - f_E|) (C2 = 2C of them); ``w`` holds the thread's 4 channels for every tap
+__device__ __forceinline__ void fusion_u4(const float (&gt)[9], const float4 (&w)[9], float (&u)[4]) {
+  u[0] = u[1] = u[2] = u[3] = 0.f;
+#pragma unroll
+  for (int t = 0; t < 9; ++t) {
+    u[0] = fmaf(w[t].x, gt[t], u[0]);
+    u[1] = fmaf(w[t].y, gt[t], u[1]);
+    u[2] = fmaf(w[t].z, gt[t], u[2]);
+    u[3] = fmaf(w[t].w, gt[t], u[3]);
+  }
+}
+
+// the 4 virtual-concat values at channel c' (= 4 * v): f_G's for c' < C, |f_G - f_E| beyond
+__device__ __forceinline__ void fusion_a4(const float* __restrict__ fg, const float* __restrict__ fe, int64_t o, int cc, bool second,
+                                          float (&a)[4]) {
+  const float4 gv = __ldg(reinterpret_cast<const float4*>(fg + o + cc));
+  if (!second) {
+    a[0] = gv.x; a[1] = gv.y; a[2] = gv.z; a[3] = gv.w;
+    return;
+  }
+  const float4 ev = __ldg(reinterpret_cast<const float4*>(fe + o + cc));
+  a[0] = fabsf(gv.x - ev.x); a[1] = fabsf(gv.y - ev.y); a[2] = fabsf(gv.z - ev.z); a[3] = fabsf(gv.w - ev.w);
+}
+
+// per (chunk, b, c'): (sum u, sum u * ahat) in double, ahat = (a - mean) * rstd.  dyn smem: pstep * C2 * 2 doubles
+__global__ void __launch_bounds__(256)
+fusion_adain_partial_kernel(const float* __restrict__ gz, const float* __restrict__ w2, const float* __restrict__ fg,
+                            const float* __restrict__ fe, const float* __restrict__ stats, int H, int W, int C, int64_t chunk,
+                            double* __restrict__ ws) {
+  extern __shared__ double sred[];
+  const int64_t HW = (int64_t)H * W;
+  const int C2 = 2 * C, b = blockIdx.y, nvec = C2 / 4, pstep = blockDim.x / nvec;
+  const int v = threadIdx.x % nvec, lane_p = threadIdx.x / nvec;
+  const int64_t p_begin = (int64_t)blockIdx.x * chunk;
+  const int64_t p_end = (p_begin + chunk < HW) ? p_begin + chunk : HW;
+  if (lane_p < pstep) {
+    const bool second = v * 4 >= C;
+    const int cc = second ? v * 4 - C : v * 4;
+    float4 w[9];
+#pragma unroll
+    for (int t = 0; t < 9; ++t) w[t] = __ldg(reinterpret_cast<const float4*>(w2 + (int64_t)t * C2 + v * 4));
+    float mean[4], rstd[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      mean[i] = stats[((int64_t)b * C2 + v * 4 + i) * 2];
+      rstd[i] = stats[((int64_t)b * C2 + v * 4 + i) * 2 + 1];
+    }
+    double sg[4] = {0, 0, 0, 0}, sgx[4] = {0, 0, 0, 0};
+    const float* gzb = gz + (int64_t)b * HW;
+    for (int64_t p = p_begin + lane_p; p < p_end; p += pstep) {
+      float gt[9], u[4], a[4];
+      fusion_taps(gzb, (int)(p / W), (int)(p % W), H, W, gt);
+      fusion_u4(gt, w, u);
+      fusion_a4(fg, fe, ((int64_t)b * HW + p) * C, cc, second, a);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        sg[i] += (double)u[i];
+        sgx[i] = fma((double)u[i], (double)((a[i] - mean[i]) * rstd[i]), sgx[i]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      sred[((int64_t)lane_p * C2 + v * 4 + i) * 2] = sg[i];
+      sred[((int64_t)lane_p * C2 + v * 4 + i) * 2 + 1] = sgx[i];
+    }
+  }
+  __syncthreads();
+  double* dst = ws + ((int64_t)blockIdx.x * gridDim.y + b) * C2 * 2;
+  for (int i = threadIdx.x; i < 2 * C2; i += blockDim.x) {
+    double s = 0.0;
+    for (int l = 0; l < pstep; ++l) s += sred[(int64_t)l * C2 * 2 + i];
+    dst[i] = s;
+  }
+}
+
+// g_fg = g_dir + T1 + sign(f_G - f_E) * T2,  g_fe = -sign(f_G - f_E) * T2 + g_p * m, with T1, T2 the AdaIN backward of the two halves
+// of the concat (channel c and C + c): gamma * rstd * ((u - m_u) - ahat * m_ua)
+__global__ void __launch_bounds__(256)
+fusion_input_grad_kernel(const float* __restrict__ gz, const float* __restrict__ w2, const float* __restrict__ fg,
+                         const float* __restrict__ fe, const float* __restrict__ stats, const float* __restrict__ gb,
+                         const float* __restrict__ sums, float inv_hw, const float* __restrict__ gdir,
+                         const float* __restrict__ gp, const float* __restrict__ m, int H, int W, int C, int64_t chunk,
+                         float* __restrict__ gfg, float* __restrict__ gfe) {
+  const int64_t HW = (int64_t)H * W;
+  const int C2 = 2 * C, b = blockIdx.y, nvec = C / 4, pstep = blockDim.x / nvec;
+  const int v = threadIdx.x % nvec, lane_p = threadIdx.x / nvec;
+  if (lane_p >= pstep) return;
+  const int64_t p_begin = (int64_t)blockIdx.x * chunk;
+  const int64_t p_end = (p_begin + chunk < HW) ? p_begin + chunk : HW;
+  float4 w1[9], w2b[9];
+#pragma unroll
+  for (int t = 0; t < 9; ++t) {
+    w1[t] = __ldg(reinterpret_cast<const float4*>(w2 + (int64_t)t * C2 + v * 4));
+    w2b[t] = __ldg(reinterpret_cast<const float4*>(w2 + (int64_t)t * C2 + C + v * 4));
+  }
+  float mean[2][4], rstd[2][4], coef[2][4], mu[2][4], mua[2][4];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = h * C + v * 4 + i;
+      const int64_t e = (int64_t)b * C2 + c;
+      mean[h][i] = stats[e * 2];
+      rstd[h][i] = stats[e * 2 + 1];
+      coef[h][i] = gb[(int64_t)b * 2 * C2 + c] * rstd[h][i];
+      mu[h][i] = sums[e * 2] * inv_hw;
+      mua[h][i] = sums[e * 2 + 1] * inv_hw;
+    }
+  const float* gzb = gz + (int64_t)b * HW;
+  for (int64_t p = p_begin + lane_p; p < p_end; p += pstep) {
+    const int y = (int)(p / W), x = (int)(p % W);
+    const int64_t o = ((int64_t)b * HW + p) * C + v * 4;
+    float gt[9], u1[4], u2[4];
+    fusion_taps(gzb, y, x, H, W, gt);
+    fusion_u4(gt, w1, u1);
+    fusion_u4(gt, w2b, u2);
+    const float4 gv = __ldg(reinterpret_cast<const float4*>(fg + o));
+    const float4 ev = __ldg(reinterpret_cast<const float4*>(fe + o));
+    const float4 pv = __ldg(reinterpret_cast<const float4*>(gp + o));
+    float4 dv = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (gdir) dv = __ldg(reinterpret_cast<const float4*>(gdir + o));
+    const float mv = __ldg(m + (int64_t)b * HW + p);
+    const float ga[4] = {gv.x, gv.y, gv.z, gv.w}, ea[4] = {ev.x, ev.y, ev.z, ev.w}, pa[4] = {pv.x, pv.y, pv.z, pv.w};
+    const float da[4] = {dv.x, dv.y, dv.z, dv.w};
+    float rg[4], re[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float d = ga[i] - ea[i];
+      const float sgn = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);
+      const float t1 = coef[0][i] * ((u1[i] - mu[0][i]) - (ga[i] - mean[0][i]) * rstd[0][i] * mua[0][i]);
+      const float t2 = coef[1][i] * ((u2[i] - mu[1][i]) - (fabsf(d) - mean[1][i]) * rstd[1][i] * mua[1][i]);
+      rg[i] = da[i] + t1 + sgn * t2;
+      re[i] = fmaf(pa[i], mv, -sgn * t2);
+    }
+    *reinterpret_cast<float4*>(gfg + o) = make_float4(rg[0], rg[1], rg[2], rg[3]);
+    *reinterpret_cast<float4*>(gfe + o) = make_float4(re[0], re[1], re[2], re[3]);
+  }
+}
+
+}  // namespace
+
+extern "C" int vt_torgb_gate_grad_nhwc(const float* g, const float* g_rgb, const float* w_rgb, int wB, int w_cstride, const float* ref,
+                                       float slope, float gain, int B, int64_t HW, int C, float* out, void* stream) {
+  VT_CHECK(g_rgb && w_rgb && ref && out, "torgb_gate_grad: null pointer");
+  VT_CHECK(B >= 1 && HW >= 1 && C >= 4 && C % 4 == 0 && w_cstride >= C && w_cstride % 4 == 0 && (wB == 1 || wB == B),
+           "torgb_gate_grad: bad shape (C %% 4 == 0, w_cstride >= C, wB 1 or B)");
+  VT_CHECK((!g || aligned16(g)) && aligned16(w_rgb) && aligned16(ref) && aligned16(out), "torgb_gate_grad: tensors must be 16-byte aligned");
+  int64_t blocks = vt_cdiv((int64_t)B * HW * (C / 4), 256);
+  const int64_t cap = (int64_t)vt_num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  torgb_gate_grad_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(g, g_rgb, w_rgb, wB, w_cstride, ref, slope, gain, B, HW,
+                                                                             C, out);
+  VT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int64_t vt_fusion_mask_grad_ws_bytes(int B, int64_t HW) {
+  if (B < 1 || HW < 1) return -1;
+  return vt_cdiv(HW, MASK_CHUNK) * B * (int64_t)sizeof(double);
+}
+
+extern "C" int vt_fusion_mask_grad_nhwc(const float* g_p, const float* f_e, const float* m, const float* g_m, int B, int64_t HW, int C,
+                                        float* g_z, float* bias_grad, void* ws, void* stream) {
+  VT_CHECK(g_p && f_e && m && g_z && bias_grad && ws, "fusion_mask_grad: null pointer");
+  VT_CHECK(B >= 1 && B <= 65535 && HW >= 1 && C >= 4 && C % 4 == 0, "fusion_mask_grad: bad shape (C must be a multiple of 4)");
+  VT_CHECK(aligned16(g_p) && aligned16(f_e) && aligned16(ws), "fusion_mask_grad: tensors must be 16-byte aligned");
+  const int64_t chunks = vt_cdiv(HW, MASK_CHUNK);
+  VT_CHECK(chunks < (1LL << 31), "fusion_mask_grad: plane too large");
+  cudaStream_t st = (cudaStream_t)stream;
+  fusion_mask_grad_kernel<<<dim3((unsigned)chunks, (unsigned)B), 256, 0, st>>>(g_p, f_e, m, g_m, HW, C, g_z, (double*)ws);
+  VT_LAUNCH_CHECK();
+  partials_sum_kernel<<<1, 256, 0, st>>>((const double*)ws, chunks * B, 1, 1.f, bias_grad);
+  VT_LAUNCH_CHECK();
+  return 0;
+}
+
+#define VT_FUSION_SHAPE_CHECK(name)                                                                                   \
+  VT_CHECK(B >= 1 && B <= 65535 && H >= 1 && W >= 1 && C >= 4 && C % 4 == 0 && C <= 512, name ": bad shape (C must be a " \
+           "multiple of 4, at most 512)")
+
+extern "C" int vt_fusion_adain_grad_stats_nhwc(const float* g_z, const float* w2, const float* f_g, const float* f_e, const float* stats,
+                                               int B, int H, int W, int C, float* sums, void* ws, void* stream) {
+  VT_CHECK(g_z && w2 && f_g && f_e && stats && sums && ws, "fusion_adain_grad_stats: null pointer");
+  VT_CHECK(aligned16(w2) && aligned16(f_g) && aligned16(f_e) && aligned16(ws), "fusion_adain_grad_stats: tensors must be 16-byte aligned");
+  VT_FUSION_SHAPE_CHECK("fusion_adain_grad_stats");
+  const int64_t HW = (int64_t)H * W;
+  int64_t chunk, chunks;
+  instnorm_plan(HW, 2 * C, &chunk, &chunks);
+  VT_CHECK(chunks < (1LL << 31), "fusion_adain_grad_stats: plane too large");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int pstep = 256 / (2 * C / 4);
+  fusion_adain_partial_kernel<<<dim3((unsigned)chunks, (unsigned)B), 256, (size_t)pstep * 2 * C * 2 * sizeof(double), st>>>(
+      g_z, w2, f_g, f_e, stats, H, W, C, chunk, (double*)ws);
+  VT_LAUNCH_CHECK();
+  const int64_t n = (int64_t)B * 2 * C * 2;
+  partials_sum_kernel<<<(unsigned)vt_cdiv(n, 8), 256, 0, st>>>((const double*)ws, chunks, n, 1.f, sums);
+  VT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int vt_fusion_input_grad_nhwc(const float* g_z, const float* w2, const float* f_g, const float* f_e, const float* stats,
+                                         const float* gamma_beta, const float* sums, const float* g_dir, const float* g_p, const float* m,
+                                         int B, int H, int W, int C, float* g_fg, float* g_fe, void* stream) {
+  VT_CHECK(g_z && w2 && f_g && f_e && stats && gamma_beta && sums && g_p && m && g_fg && g_fe, "fusion_input_grad: null pointer");
+  VT_CHECK(aligned16(w2) && aligned16(f_g) && aligned16(f_e) && aligned16(g_p) && (!g_dir || aligned16(g_dir)) && aligned16(g_fg) &&
+           aligned16(g_fe), "fusion_input_grad: tensors must be 16-byte aligned");
+  VT_FUSION_SHAPE_CHECK("fusion_input_grad");
+  const int64_t HW = (int64_t)H * W;
+  int64_t chunk, chunks;
+  instnorm_plan(HW, C, &chunk, &chunks);
+  VT_CHECK(chunks < (1LL << 31), "fusion_input_grad: plane too large");
+  fusion_input_grad_kernel<<<dim3((unsigned)chunks, (unsigned)B), 256, 0, (cudaStream_t)stream>>>(
+      g_z, w2, f_g, f_e, stats, gamma_beta, sums, (float)(1.0 / (double)HW), g_dir, g_p, m, H, W, C, chunk, g_fg, g_fe);
+  VT_LAUNCH_CHECK();
   return 0;
 }
 

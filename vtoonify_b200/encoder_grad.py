@@ -97,8 +97,10 @@ def _weight_grad(conv, g_pre, x, stride, pad, dil):
     return weight_grad_nhwc(g_pre, x, Cout, Cin, k, k, stride, (pad, pad), (dil, dil)).reshape(conv.weight.shape)
 
 
-def _backward(model, rec, feat, g_feat, g_skip, need, x_channels):
-    """-> (grad of x or None, {parameter: grad}) for the records of :func:`_forward_train`; ``need(p)``: p wants a gradient."""
+def _backward(model, rec, feat, g_feat, g_skip, need, x_channels, g_inject=None):
+    """-> (grad of x or None, {parameter: grad}) for the records of :func:`_forward_train`; ``need(p)``: p wants a gradient.
+    ``g_inject`` {id(activation): NHWC gradient}: more gradient reaching an encoder block's output from outside the encoder (the
+    fusion modules read ``encoder_features``), added before that block's gate."""
     grads = {}
     enc5 = model.encoder[-1]
     B, H, W, C = feat.shape
@@ -134,6 +136,8 @@ def _backward(model, rec, feat, g_feat, g_skip, need, x_channels):
             g = _input_grad(blk.conv, 1.0, gp1, H, W, 1, 1, 1, res=g, beta=_R2)   # + the skip term g / sqrt(2)
         else:
             _, conv, slope, x, y = r
+            if g_inject and id(y) in g_inject:
+                g = ops.axpby(g, g_inject[id(y)], 1.0, 1.0, round_tf32=False)
             gp, db = ops.act_grad(g, ref=y, slope=slope, gain=1.0, bias_grad=True)
             grads[conv.bias] = db
             if need(conv.weight):

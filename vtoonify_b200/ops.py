@@ -885,6 +885,18 @@ def act_grad(g: torch.Tensor, ref: Optional[torch.Tensor] = None, slope: float =
     return (out, bg) if bias_grad else out
 
 
+def channel_sum_nhwc(g: torch.Tensor) -> torch.Tensor:
+    """Per-channel sum ``[C]`` of a contiguous NHWC ``[B, H, W, C]`` tensor (a bias gradient): the reduction of :func:`act_grad`
+    without its elementwise output (deterministic, double-precision partials)."""
+    _req_cuda(g)
+    _nhwc_check("channel_sum_nhwc", g, g)
+    B, H, W, C = g.shape
+    bg = torch.empty((C,), device=g.device, dtype=torch.float32)
+    check(_lib.load().vt_act_grad_nhwc(g.data_ptr(), None, 0.2, 1.0, None, 1.0, None, None, None, None, B, H * W, C, None,
+                                       bg.data_ptr(), _grad_ws(B, H * W, C, g.device).data_ptr(), _stream()))
+    return bg
+
+
 def mbstd(x: torch.Tensor, group: int) -> torch.Tensor:
     """Minibatch standard deviation of the StyleGAN discriminator (model/vtoonify.py:67-75) on NHWC ``x`` [B, H, W, C]:
     ``[B, H, W, pad32(C + 1)]`` holding x, then the statistic of the sample's column ``b % (B / group)``, then zeros."""
@@ -910,6 +922,80 @@ def mbstd_grad(g: torch.Tensor, x: torch.Tensor, group: int) -> torch.Tensor:
     out = torch.empty_like(x)
     check(_lib.load().vt_mbstd_grad_nhwc_f32(g.data_ptr(), x.data_ptr(), out.data_ptr(), B, group, H * W, C, g.shape[3], _stream()))
     return out
+
+
+def torgb_gate_grad(g: Optional[torch.Tensor], g_rgb: torch.Tensor, w_rgb: torch.Tensor, ref: torch.Tensor, slope: float = 0.2,
+                    gain: float = SQRT2) -> torch.Tensor:
+    """Backward of a StyledConv whose activation ``ref`` (NHWC [B, H, W, C]) also feeds a 1x1 ToRGB: ``gate(ref) * gain * (g +
+    w_rgb[b]^T g_rgb)``.  ``g``: the activation's other gradient (None: 0); ``g_rgb``: the planar image gradient [B, 3, H, W], read
+    as it is; ``w_rgb``: ToRGB's modulated weights [wB, 1, 3, c] (c >= C)."""
+    _req_cuda(g, g_rgb, w_rgb, ref)
+    _nhwc_check("torgb_gate_grad", ref, g, ref)
+    B, H, W, C = ref.shape
+    if tuple(g_rgb.shape) != (B, 3, H, W) or w_rgb.dim() != 4 or tuple(w_rgb.shape[1:3]) != (1, 3) or w_rgb.shape[0] not in (1, B):
+        raise _lib.VtError("torgb_gate_grad: g_rgb must be [B, 3, H, W] and w_rgb [1 or B, 1, 3, c]")
+    w_rgb, g_rgb = w_rgb.contiguous(), g_rgb.contiguous()
+    out = torch.empty_like(ref)
+    check(_lib.load().vt_torgb_gate_grad_nhwc(_ptr(g), g_rgb.data_ptr(), w_rgb.data_ptr(), w_rgb.shape[0], w_rgb.shape[3],
+                                              ref.data_ptr(), slope, gain, B, H * W, C, out.data_ptr(), _stream()))
+    return out
+
+
+def fusion_mask_grad(g_p: torch.Tensor, f_e: torch.Tensor, m: torch.Tensor, g_m: Optional[torch.Tensor] = None):
+    """Fusion's mask head ``m = tanh(relu z)`` read by ``f_E * m``: ``g_p`` (gradient of ``f_E * m``), ``f_e`` NHWC [B, H, W, C],
+    ``m`` and ``g_m`` (the returned mask's own gradient, may be None) planar [B, 1, H, W] -> (g_z [B, 1, H, W], conv2's bias gradient [1])."""
+    _req_cuda(g_p, f_e, m, g_m)
+    _nhwc_check("fusion_mask_grad", f_e, g_p, f_e)
+    B, H, W, C = f_e.shape
+    for t in (m, g_m):
+        if t is not None and (t.numel() != B * H * W or not t.is_contiguous()):
+            raise _lib.VtError("fusion_mask_grad: m and g_m must be contiguous [B, 1, H, W] maps")
+    lib = _lib.load()
+    ws = torch.empty((lib.vt_fusion_mask_grad_ws_bytes(B, H * W) // 8,), device=f_e.device, dtype=torch.float64)
+    g_z = torch.empty((B, 1, H, W), device=f_e.device, dtype=torch.float32)
+    db = torch.empty((1,), device=f_e.device, dtype=torch.float32)
+    check(lib.vt_fusion_mask_grad_nhwc(g_p.data_ptr(), f_e.data_ptr(), m.data_ptr(), _ptr(g_m), B, H * W, C, g_z.data_ptr(),
+                                       db.data_ptr(), ws.data_ptr(), _stream()))
+    return g_z, db
+
+
+def _fusion_check(name, g_z, w2, f_g, f_e, stats):
+    _nhwc_check(name, f_g, f_g, f_e)
+    B, H, W, C = f_g.shape
+    if (tuple(g_z.shape) != (B, 1, H, W) or not g_z.is_contiguous() or tuple(w2.shape) != (9, 2 * C) or not w2.is_contiguous()
+            or tuple(stats.shape) != (B, 2 * C, 2) or not stats.is_contiguous()):
+        raise _lib.VtError(f"{name}: g_z must be [B, 1, H, W], w2 [9, 2C] and stats [B, 2C, 2], contiguous")
+    return B, H, W, C
+
+
+def fusion_adain_grad_stats(g_z: torch.Tensor, w2: torch.Tensor, f_g: torch.Tensor, f_e: torch.Tensor, stats: torch.Tensor) -> torch.Tensor:
+    """AdaIN-backward sums of Fusion's mask head over the virtual concat ``cat(f_G, |f_G - f_E|)``: ``[B, 2C, 2]`` = (sum of u, sum of
+    u * ahat) per plane, u = conv2's input gradient (its transposed 3x3 of ``g_z``, recomputed per pixel), ``w2`` = conv2's weight as
+    ``[9, 2C]`` (tap-major).  The two sums are also dbeta and dgamma of the affine."""
+    _req_cuda(g_z, w2, f_g, f_e, stats)
+    B, H, W, C = _fusion_check("fusion_adain_grad_stats", g_z, w2, f_g, f_e, stats)
+    sums = torch.empty((B, 2 * C, 2), device=f_g.device, dtype=torch.float32)
+    check(_lib.load().vt_fusion_adain_grad_stats_nhwc(g_z.data_ptr(), w2.data_ptr(), f_g.data_ptr(), f_e.data_ptr(), stats.data_ptr(),
+                                                      B, H, W, C, sums.data_ptr(), _grad_ws(B, H * W, 2 * C, f_g.device).data_ptr(),
+                                                      _stream()))
+    return sums
+
+
+def fusion_input_grad(g_z: torch.Tensor, w2: torch.Tensor, f_g: torch.Tensor, f_e: torch.Tensor, stats: torch.Tensor,
+                      gamma_beta: torch.Tensor, sums: torch.Tensor, g_dir: Optional[torch.Tensor], g_p: torch.Tensor, m: torch.Tensor):
+    """-> (g_{f_G}, g_{f_E}) of Fusion's mask head: the AdaIN backward of both concat halves (``sums`` from
+    :func:`fusion_adain_grad_stats`, ``gamma_beta`` [B, 4C]), the ``|f_G - f_E|`` split (sign(0) = 0), ``g_dir`` (f_G's gradient from
+    the fusion convolution, may be None) and ``g_p * m`` (``g_p``: gradient of ``f_E * m``)."""
+    _req_cuda(g_z, w2, f_g, f_e, stats, gamma_beta, sums, g_dir, g_p, m)
+    B, H, W, C = _fusion_check("fusion_input_grad", g_z, w2, f_g, f_e, stats)
+    _nhwc_check("fusion_input_grad", f_g, g_dir, g_p)
+    if tuple(gamma_beta.shape) != (B, 4 * C) or tuple(sums.shape) != (B, 2 * C, 2) or m.numel() != B * H * W or not m.is_contiguous():
+        raise _lib.VtError("fusion_input_grad: gamma_beta must be [B, 4C], sums [B, 2C, 2] and m [B, 1, H, W]")
+    g_fg, g_fe = torch.empty_like(f_g), torch.empty_like(f_e)
+    check(_lib.load().vt_fusion_input_grad_nhwc(g_z.data_ptr(), w2.data_ptr(), f_g.data_ptr(), f_e.data_ptr(), stats.data_ptr(),
+                                                gamma_beta.contiguous().data_ptr(), sums.contiguous().data_ptr(), _ptr(g_dir),
+                                                g_p.data_ptr(), m.data_ptr(), B, H, W, C, g_fg.data_ptr(), g_fe.data_ptr(), _stream()))
+    return g_fg, g_fe
 
 
 def affine_fold_weights(w: torch.Tensor, stats: torch.Tensor, gamma_beta: torch.Tensor):

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 from torch import nn
 
-from . import discriminator, encoder_grad, ops
+from . import discriminator, encoder_grad, ops, vtoonify_grad
 from ._lib import ACT_LRELU, ACT_NONE, ACT_RELU_TANH
 from .dualstylegan import AdaptiveInstanceNorm, AdaResBlock, DualStyleGAN, Linear
 from .stylegan import ConvLayer, EqualLinear, Generator, ResBlock, _PreppedWeight
@@ -198,14 +198,16 @@ class Fusion(nn.Module):
         # applies each LeakyReLU once, the fast path below fuses them into the Linear launches (act=2)
         self.linear = nn.Sequential(Linear(1, 64), LeakyReLU(0.2), Linear(64, 128), LeakyReLU(0.2))
 
-    def forward_nhwc(self, f_G, f_E, d_s=1):
+    def forward_nhwc(self, f_G, f_E, d_s=1, rec=None):
+        """``rec`` (a dict): take the route that writes ``f_E * m_E`` and keep the statistics and gamma|beta rows of the AdaIN for the
+        backward (vtoonify_grad)."""
         B = f_G.shape[0]
 
         def make_gb():   # depends on d_s only: once per (style, d_s) scope
             label = torch.full((B, 1), float(d_s), device=f_G.device, dtype=torch.float32)
             label = self.linear[2](self.linear[0](label, act=2), act=2)   # LeakyReLU(0.2) fused into the Linear launches
             return self.norm.style(label)
-        gb = ops.style_cached(self, "gb", make_gb, extra=(B, float(d_s)))
+        gb = ops.style_cached(self, "gb", make_gb, extra=(B, float(d_s)) + tuple(p._version for p in self.parameters()))
         # AdaIN(cat(f_G, |f_G - f_E|)) is never materialised: plane statistics in one pass over (f_G, f_E), the affine
         # folded into per-sample mask-conv weights, and the mask conv reads f_G / f_E directly (virtual concat)
         stats = ops.instnorm_stats(f_G, f_E)
@@ -213,7 +215,9 @@ class Fusion(nn.Module):
         w_plain = self.conv2._wp.get(self.conv2.weight, 1.0, C2, round_tf32=False)          # [1, 9, 1, 2C]
         w_fold, k_fold = ops.affine_fold_weights(w_plain, stats, gb)
         B, H, W, _ = f_G.shape
-        if ops.scale_fusable():
+        if rec is not None:
+            rec.update(stats=stats, gb=gb)
+        if ops.scale_fusable() and rec is None:
             # f_E * m_E (model/vtoonify.py:127) is never written: the fusion conv multiplies f_E tiles by m_E while it splits
             # them for the tensor cores, and fusion_skip's 3-channel conv scales its loads (VToonify.forward)
             m_E = ops.smalln_conv(f_G, w_fold, ops.conv_taps(3, 1), 1, B, H, W, bias=self.conv2.bias, act=ACT_RELU_TANH,
@@ -308,6 +312,8 @@ class VToonify(ops.WeightsEpochMixin, nn.Module):
         adastyles, resstyles = ops.style_cached(self, "styles", lambda: self._styles(style))
         if return_feat and encoder_grad.takes_autograd(self, x):
             return encoder_grad.feat_with_grad(self, x, style, d_s, resstyles)
+        if not return_feat and vtoonify_grad.takes_autograd(self, x):
+            return vtoonify_grad.forward_with_grad(self, x, style, d_s, adastyles, resstyles, return_mask)
 
         # encoder: downsampling conv blocks, then the res blocks (interleaved with dilated ModRes for D)
         feat = ops.to_nhwc(x, ops._pad32(x.shape[1]))

@@ -380,6 +380,23 @@ int vt_bilinear_add_nhwc(const float* x, const float* y, float* out, int B, int 
 int vt_frame_s2d_f32(const float* in, float* out, int B, int Hin, int Win, int Ho, int Wo, int cpad, int upsample2, void* stream);
 /* nn.MaxPool2d(3, 2, 1) on NHWC: out [B, (H-1)/2+1, (W-1)/2+1, C] */
 int vt_maxpool3x3s2_nhwc_f32(const float* in, float* out, int B, int H, int W, int C, void* stream);
+/* ---- LPIPS perceptual loss (model/stylegan/lpips, VGG16 net-lin) ---- */
+/* nn.MaxPool2d(2, 2) on NHWC: out [B, H/2, W/2, C] (floor; bit-identical to torch) */
+int vt_maxpool2x2_nhwc_f32(const float* in, float* out, int B, int H, int W, int C, void* stream);
+/* its adjoint: gx [B, H, W, C] = add + the gradient g [B, H/2, W/2, C] routed to the first maximal element of each window of the pool
+ * input x in row-major order (torch's tie rule, recomputed from x); rows / columns dropped by the floor get add alone (add may be
+ * NULL: 0) */
+int vt_maxpool2x2_grad_nhwc_f32(const float* g, const float* x, const float* add, float* gx, int B, int H, int W, int C, void* stream);
+/* bytes of the ws of vt_lpips_head_nhwc for taps of HW[k] pixels */
+int64_t vt_lpips_head_ws_bytes(int B, int n_taps, const int64_t* HW);
+/* out[b] = sum over the taps k of mean over the HW[k] pixels of sum_c w[k][c] (u0_c - u1_c)^2, u = f / (||f||_2 + 1e-10) with f0 the
+ * row of sample b and f1 that of sample B + b in f[k] (NHWC [2B, HW[k], C[k]]); 1 to 8 taps, deterministic (double partials) */
+int vt_lpips_head_nhwc(int n_taps, const float* const* f, const float* const* w, const int64_t* HW, const int* C, int B, float* out,
+                       void* ws, void* stream);
+/* the head's gradient for one tap, scaled by g_b[b] / HW: into the f0 rows (g_target, [B, HW, C]) and/or the f1 rows (g_pred); either may
+ * be NULL; 0 at a pixel whose row is all zero */
+int vt_lpips_head_grad_nhwc(const float* f, const float* w, const float* g_b, int B, int64_t HW, int C, float* g_target, float* g_pred,
+                            void* stream);
 /* F.interpolate(in, (H, W), mode='nearest') on NHWC */
 int vt_resize_nearest_nhwc_f32(const float* in, float* out, int B, int h, int w, int H, int W, int C, void* stream);
 /* out[b,c,y,x] = scale * F.interpolate(logits, (Hf, Wf), 'bilinear', align_corners=True)[b, c, step*y, step*x];

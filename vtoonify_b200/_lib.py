@@ -108,6 +108,11 @@ SYMBOLS = {
     "vt_instnorm_stats_nhwc": (c_int, [_P, _P, c_int, c_int, c_int64, c_int, c_int, c_float, _P, _P, _P]),
     "vt_frame_s2d_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "vt_maxpool3x3s2_nhwc_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+    "vt_maxpool2x2_nhwc_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+    "vt_maxpool2x2_grad_nhwc_f32": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    "vt_lpips_head_ws_bytes": (c_int64, [c_int, c_int, POINTER(c_int64)]),
+    "vt_lpips_head_nhwc": (c_int, [c_int, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int64), POINTER(c_int), c_int, _P, _P, _P]),
+    "vt_lpips_head_grad_nhwc": (c_int, [_P, _P, _P, c_int, c_int64, c_int, _P, _P, _P]),
     "vt_resize_nearest_nhwc_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "vt_logits_readout_f32": (c_int, [_P, _P] + [c_int] * 10 + [c_float, c_int64, _P]),
     "vt_adain_affine_f32": (c_int, [_P, _P, _P, c_int, c_int, _P]),

@@ -77,6 +77,79 @@ maxpool3x3s2_kernel(const float* __restrict__ in, float* __restrict__ out, int H
   }
 }
 
+// nn.MaxPool2d(2, 2) on NHWC (VGG16 of the LPIPS loss); the last row / column of an odd map is dropped
+__global__ void __launch_bounds__(256)
+maxpool2x2_kernel(const float* __restrict__ in, float* __restrict__ out, int H, int W, int C, int Ho, int Wo) {
+  const int b = blockIdx.y, nvec = C / 4;
+  const int64_t total = (int64_t)Ho * Wo * nvec;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % nvec) * 4;
+    const int64_t p = i / nvec;
+    const int ox = (int)(p % Wo), oy = (int)(p / Wo);
+    const float* r0 = in + (((int64_t)b * H + 2 * oy) * W + 2 * ox) * C + c;
+    const float4 a = __ldg(reinterpret_cast<const float4*>(r0)), bq = __ldg(reinterpret_cast<const float4*>(r0 + C));
+    const float4 cq = __ldg(reinterpret_cast<const float4*>(r0 + (int64_t)W * C));
+    const float4 d = __ldg(reinterpret_cast<const float4*>(r0 + (int64_t)W * C + C));
+    float4 m;
+    m.x = fmaxf(fmaxf(a.x, bq.x), fmaxf(cq.x, d.x)); m.y = fmaxf(fmaxf(a.y, bq.y), fmaxf(cq.y, d.y));
+    m.z = fmaxf(fmaxf(a.z, bq.z), fmaxf(cq.z, d.z)); m.w = fmaxf(fmaxf(a.w, bq.w), fmaxf(cq.w, d.w));
+    *reinterpret_cast<float4*>(out + (((int64_t)b * Ho + oy) * Wo + ox) * C + c) = m;
+  }
+}
+
+// the window element that receives the gradient: the first maximal one in row-major order, as ATen's max_pool2d records it
+__device__ __forceinline__ void maxpool2x2_route(float a, float b, float c, float d, float g, float (&o)[4]) {
+  const float m = fmaxf(fmaxf(a, b), fmaxf(c, d));
+  const int k = a == m ? 0 : (b == m ? 1 : (c == m ? 2 : 3));
+#pragma unroll
+  for (int j = 0; j < 4; ++j) o[j] = j == k ? g : 0.f;
+}
+
+// Adjoint of maxpool2x2_kernel, one thread per (window, 4 channels): the argmax is recomputed from the pool input x (no index
+// tensor); add (may be NULL) is added to every input position, and rows / columns dropped by the floor get add (or 0) alone.
+__global__ void __launch_bounds__(256)
+maxpool2x2_grad_kernel(const float* __restrict__ g, const float* __restrict__ x, const float* __restrict__ add, float* __restrict__ gx,
+                       int H, int W, int C, int Ho, int Wo) {
+  const int b = blockIdx.y, nvec = C / 4;
+  const int64_t total = (int64_t)Ho * Wo * nvec;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % nvec) * 4;
+    const int64_t p = i / nvec;
+    const int ox = (int)(p % Wo), oy = (int)(p / Wo);
+    int64_t off[4];
+    off[0] = (((int64_t)b * H + 2 * oy) * W + 2 * ox) * C + c;
+    off[1] = off[0] + C;
+    off[2] = off[0] + (int64_t)W * C;
+    off[3] = off[2] + C;
+    float4 v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = __ldg(reinterpret_cast<const float4*>(x + off[j]));
+    const float4 gv = __ldg(reinterpret_cast<const float4*>(g + (((int64_t)b * Ho + oy) * Wo + ox) * C + c));
+    float o[4][4];   // [channel][window element]
+    maxpool2x2_route(v[0].x, v[1].x, v[2].x, v[3].x, gv.x, o[0]);
+    maxpool2x2_route(v[0].y, v[1].y, v[2].y, v[3].y, gv.y, o[1]);
+    maxpool2x2_route(v[0].z, v[1].z, v[2].z, v[3].z, gv.z, o[2]);
+    maxpool2x2_route(v[0].w, v[1].w, v[2].w, v[3].w, gv.w, o[3]);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float4 r = make_float4(o[0][j], o[1][j], o[2][j], o[3][j]);
+      if (add) {
+        const float4 s = __ldg(reinterpret_cast<const float4*>(add + off[j]));
+        r.x += s.x; r.y += s.y; r.z += s.z; r.w += s.w;
+      }
+      *reinterpret_cast<float4*>(gx + off[j]) = r;
+    }
+    // the floor's dropped last column / row (and their corner) are written by the windows next to them
+    const bool col = (W & 1) && ox == Wo - 1, row = (H & 1) && oy == Ho - 1;
+    auto pass = [&](int64_t o) {
+      *reinterpret_cast<float4*>(gx + o) = add ? __ldg(reinterpret_cast<const float4*>(add + o)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    };
+    if (col) { pass(off[1] + C); pass(off[3] + C); }
+    if (row) { pass(off[2] + (int64_t)W * C); pass(off[3] + (int64_t)W * C); }
+    if (col && row) pass(off[3] + (int64_t)W * C + C);
+  }
+}
+
 // F.interpolate(x, (H, W), mode='nearest') on NHWC: src = min(floor(dst * in/out), in - 1) with the scale in fp32 (ATen)
 __global__ void __launch_bounds__(256)
 resize_nearest_kernel(const float* __restrict__ in, float* __restrict__ out, int h, int w, int H, int W, int C) {
@@ -144,6 +217,26 @@ extern "C" int vt_maxpool3x3s2_nhwc_f32(const float* in, float* out, int B, int 
   VT_CHECK(in && out && B >= 1 && B <= 65535 && H >= 1 && W >= 1 && C >= 4 && C % 4 == 0, "maxpool3x3s2: bad args");
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;   // floor((H + 2 - 3) / 2) + 1
   maxpool3x3s2_kernel<<<dim3(grid1((int64_t)Ho * Wo * (C / 4), 256), (unsigned)B), 256, 0, (cudaStream_t)stream>>>(in, out, H, W, C, Ho, Wo);
+  VT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int vt_maxpool2x2_nhwc_f32(const float* in, float* out, int B, int H, int W, int C, void* stream) {
+  VT_CHECK(in && out && B >= 1 && B <= 65535 && H >= 2 && W >= 2 && C >= 4 && C % 4 == 0, "maxpool2x2: bad args");
+  VT_CHECK((((uintptr_t)in | (uintptr_t)out) & 15) == 0, "maxpool2x2: tensors must be 16-byte aligned");
+  const int Ho = H / 2, Wo = W / 2;
+  maxpool2x2_kernel<<<dim3(grid1((int64_t)Ho * Wo * (C / 4), 256), (unsigned)B), 256, 0, (cudaStream_t)stream>>>(in, out, H, W, C, Ho, Wo);
+  VT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int vt_maxpool2x2_grad_nhwc_f32(const float* g, const float* x, const float* add, float* gx, int B, int H, int W, int C,
+                                           void* stream) {
+  VT_CHECK(g && x && gx && B >= 1 && B <= 65535 && H >= 2 && W >= 2 && C >= 4 && C % 4 == 0, "maxpool2x2_grad: bad args");
+  VT_CHECK((((uintptr_t)g | (uintptr_t)x | (uintptr_t)add | (uintptr_t)gx) & 15) == 0, "maxpool2x2_grad: tensors must be 16-byte aligned");
+  const int Ho = H / 2, Wo = W / 2;
+  maxpool2x2_grad_kernel<<<dim3(grid1((int64_t)Ho * Wo * (C / 4), 256), (unsigned)B), 256, 0, (cudaStream_t)stream>>>(g, x, add, gx, H, W,
+                                                                                                                    C, Ho, Wo);
   VT_LAUNCH_CHECK();
   return 0;
 }

@@ -1162,6 +1162,72 @@ def maxpool3x3s2(x: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def maxpool2x2(x: torch.Tensor) -> torch.Tensor:
+    """``nn.MaxPool2d(2, 2)`` on NHWC ``[B, H, W, C]`` -> ``[B, H // 2, W // 2, C]`` (bit-identical to torch's)."""
+    _req_cuda(x)
+    B, H, W, C = x.shape
+    out = torch.empty((B, H // 2, W // 2, C), device=x.device, dtype=torch.float32)
+    check(_lib.load().vt_maxpool2x2_nhwc_f32(x.contiguous().data_ptr(), out.data_ptr(), B, H, W, C, _stream()))
+    return out
+
+
+def maxpool2x2_grad(g: torch.Tensor, x: torch.Tensor, add: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Adjoint of :func:`maxpool2x2`: ``g`` [B, H // 2, W // 2, C] goes to the first maximal element of each window of the pool input
+    ``x`` in row-major order (torch's tie rule); ``add`` (``x``'s shape, may be None) is added to the result."""
+    _req_cuda(g, x, add)
+    _nhwc_check("maxpool2x2_grad", x, x, add)
+    B, H, W, C = x.shape
+    if tuple(g.shape) != (B, H // 2, W // 2, C) or not g.is_contiguous():
+        raise _lib.VtError(f"maxpool2x2_grad: g {tuple(g.shape)} must be contiguous [B, H // 2, W // 2, C] of x {tuple(x.shape)}")
+    out = torch.empty_like(x)
+    check(_lib.load().vt_maxpool2x2_grad_nhwc_f32(g.data_ptr(), x.data_ptr(), _ptr(add), out.data_ptr(), B, H, W, C, _stream()))
+    return out
+
+
+def lpips_head(taps: Sequence[torch.Tensor], lin_w: Sequence[torch.Tensor]) -> torch.Tensor:
+    """LPIPS head over NHWC taps ``[2B, h_k, w_k, C_k]`` (rows ``b`` and ``B + b`` are the two images of pair ``b``) with the ``lin``
+    weights ``[C_k]`` -> ``[B]``: the sum over the taps of the spatial mean of ``sum_c w_c (u0_c - u1_c)^2``, u = f / (||f|| + 1e-10).
+    Deterministic: reruns are bit-identical."""
+    if len(taps) != len(lin_w) or not taps:
+        raise _lib.VtError("lpips_head: one lin weight per tap")
+    _req_cuda(*taps, *lin_w)
+    B2 = taps[0].shape[0]
+    if B2 % 2:
+        raise _lib.VtError("lpips_head: taps must hold 2B rows")
+    for t, w in zip(taps, lin_w):
+        if t.dim() != 4 or t.shape[0] != B2 or not t.is_contiguous() or w.numel() != t.shape[3] or not w.is_contiguous():
+            raise _lib.VtError("lpips_head: taps must be contiguous NHWC [2B, h, w, C] with contiguous [C] weights")
+    n, B = len(taps), B2 // 2
+    hw = (_lib.c_int64 * n)(*[t.shape[1] * t.shape[2] for t in taps])
+    cs = (_lib.c_int * n)(*[t.shape[3] for t in taps])
+    fp = (_lib.c_void_p * n)(*[t.data_ptr() for t in taps])
+    wp = (_lib.c_void_p * n)(*[w.data_ptr() for w in lin_w])
+    lib = _lib.load()
+    nbytes = lib.vt_lpips_head_ws_bytes(B, n, hw)
+    if nbytes < 0:
+        raise _lib.VtError("lpips_head: bad tap shapes")
+    ws = torch.empty((nbytes // 8,), device=taps[0].device, dtype=torch.float64)
+    out = torch.empty((B,), device=taps[0].device, dtype=torch.float32)
+    check(lib.vt_lpips_head_nhwc(n, fp, wp, hw, cs, B, out.data_ptr(), ws.data_ptr(), _stream()))
+    return out
+
+
+def lpips_head_grad(tap: torch.Tensor, lin_w: torch.Tensor, g_b: torch.Tensor, target: bool, pred: bool):
+    """Gradient of :func:`lpips_head` for one tap ``[2B, h, w, C]``, scaled by ``g_b`` [B] (the loss gradient per sample) -> NHWC
+    ``[nb * B, h, w, C]``: the target rows (0..B-1) then the pred rows (B..2B-1) of whichever of the two are asked for."""
+    _req_cuda(tap, lin_w, g_b)
+    B2, h, w, C = tap.shape
+    B = B2 // 2
+    if B2 % 2 or not tap.is_contiguous() or lin_w.numel() != C or g_b.numel() != B or not (target or pred):
+        raise _lib.VtError("lpips_head_grad: tap must be contiguous [2B, h, w, C], lin_w [C] and g_b [B]; ask for a side")
+    out = torch.empty(((int(target) + int(pred)) * B, h, w, C), device=tap.device, dtype=torch.float32)
+    gt = out[:B] if target else None
+    gp = out[B:] if (target and pred) else (out if pred else None)
+    check(_lib.load().vt_lpips_head_grad_nhwc(tap.data_ptr(), lin_w.contiguous().data_ptr(), g_b.contiguous().data_ptr(), B, h * w, C,
+                                              _ptr(gt), _ptr(gp), _stream()))
+    return out
+
+
 def resize_nearest(x: torch.Tensor, H: int, W: int) -> torch.Tensor:
     _req_cuda(x)
     B, h, w, C = x.shape

@@ -39,6 +39,10 @@ def det_tensor(key: str, ref: torch.Tensor, seed: int = 0) -> torch.Tensor:
         return 0.25 + 0.05 * r                                   # PReLU slopes
     if key.endswith("blur.kernel") or key.endswith("upsample.kernel") or key.endswith(".0.kernel"):
         return ref.detach().clone().float()                      # FIR taps are architecture constants
+    if key in ("scaling_layer.shift", "scaling_layer.scale"):
+        return ref.detach().clone().float()                      # LPIPS input normalisation: constants
+    if re.fullmatch(r"lin\d\.model\.1\.weight", key):
+        return 0.1 * r.abs()                                     # LPIPS lin weights are non-negative (the released ones average 0.09)
     if DISCRIMINATOR_EQUAL_WEIGHT.search(key):
         return r                                                 # ConditionalDiscriminator's EqualConv2d / EqualLinear weights:
                                                                  # randn, as the reference initialises them (the layer's own

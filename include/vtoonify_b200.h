@@ -405,6 +405,18 @@ int vt_resize_nearest_nhwc_f32(const float* in, float* out, int B, int h, int w,
 int vt_logits_readout_f32(const float* in, float* out, int B, int h, int w, int c_stride, int n_classes, int Hf, int Wf,
                           int Ho, int Wo, int step, float scale, int64_t out_bstride, void* stream);
 
+/* ---- training-data augmentation (model/simple_augment.py random_apply_affine) ---- */
+/* host only: the tile side (16 or 8) of vt_augment_affine_f32 for the per-sample warp coefficients coef (host, [B][6] double: x2-image
+ * x = c0 + c1 j + c2 i, y = c3 + c4 j + c5 i at warp-grid column j, row i), chosen so the worst sample's footprint fits shared memory,
+ * or 0 when none fits or a coordinate leaves +-2^22 (the caller then runs the unfused statements); win (may be NULL) receives the
+ * x2-image window (width, height) to pass to the launch; -1 on bad arguments */
+int vt_augment_affine_plan(const double* coef, int B, int H, int W, int* win);
+/* out [B,C,H,W] = the 12-tap x2 down (flipped kernel, crop 1) of the bilinear warp (zeros outside) over the 2(H+6) x 2(W+6) warp grid
+ * of the 12-tap x2 up (zeros beyond the padded extent) of in [B,C,H,W] reflect-padded to [Hp, Wp] with pads (pad_y, pad_x) at the
+ * top-left; planar fp32, kernel: 12 device floats, coef: device [B][6] double; tile / win from vt_augment_affine_plan; one launch */
+int vt_augment_affine_f32(const float* in, float* out, const float* kernel, const double* coef, int B, int C, int H, int W, int pad_x,
+                          int pad_y, int Hp, int Wp, int tile, int win_w, int win_h, void* stream);
+
 /* ---- elementwise helpers ------------------------------------------------------------------ */
 /* out = a * scale_a + b * scale_b (b may be NULL) */
 int vt_axpby_f32(const float* a, const float* b, float* out, int64_t n, float scale_a, float scale_b, int round_tf32, void* stream);

@@ -417,6 +417,37 @@ int vt_augment_affine_plan(const double* coef, int B, int H, int W, int* win);
 int vt_augment_affine_f32(const float* in, float* out, const float* kernel, const double* coef, int B, int C, int H, int W, int pad_x,
                           int pad_y, int Hp, int Wp, int tile, int win_w, int win_h, void* stream);
 
+/* ---- RAFT optical flow (model/raft/core, full model, eval; vtoonify_b200.raft) ---- */
+/* out [nB, H/2, W/2, cpad] (nB = B, or 2B when img2 is non-NULL: image2's rows follow image1's) = the space-to-depth tensor
+ * Z[y, x, (py*2+px)*3 + c] of X = 2 * (img / 255) - 1 (planar [B, 3, H, W] in 0..255), zero pad channels; H, W even */
+int vt_raft_input_s2d_f32(const float* img1, const float* img2, float* out, int B, int H, int W, int cpad, void* stream);
+/* NHWC [B, HW, C]: out = relu((x - mean) * rstd), and with res: relu(that + s), s = res, or (res - mean') * rstd' when stats_res is
+ * non-NULL; stats / stats_res: [B, C, 2] (mean, rstd) */
+int vt_raft_norm_relu_nhwc(const float* x, const float* stats, const float* res, const float* stats_res, float* out, int B, int64_t HW,
+                           int C, void* stream);
+/* cnet [npix, 2C] -> net [npix, C] = tanh(cnet[:, :C]) and inp[p * inp_cpitch + c] = relu(cnet[p, C + c]) */
+int vt_raft_context_f32(const float* cnet, float* net, float* inp, int64_t npix, int C, int inp_cpitch, void* stream);
+/* F.avg_pool2d(2, 2) of N rows [h, w] (row stride in_stride floats) -> dense [N, h/2, w/2] (floor), torch's summation order */
+int vt_raft_corr_pool_f32(const float* in, float* out, int64_t N, int h, int w, int64_t in_stride, void* stream);
+/* CorrBlock lookup, radius 4, 4 levels: level l has size (h2 >> l, w2 >> l) per row (levels[l], row stride strides[l]; row p belongs to
+ * the coords [npix, 2] (x, y) entry p); out[p * out_cpitch + l*81 + 9i + j] = bilinear sample at coords[p] / 2^l + (i - 4, j - 4),
+ * zeros outside (grid_sample, align_corners=True) */
+int vt_raft_corr_lookup_f32(const float* const* levels, const int64_t* strides, int h2, int w2, const float* coords, float* out,
+                            int out_cpitch, int64_t npix, void* stream);
+/* out [B, h, w, Cout] = relu(bias + 7x7 convolution (zero padding 3) of the flow coords - grid); w: [7*7][2][Cout] */
+int vt_raft_convf1_f32(const float* coords, const float* w, const float* bias, float* out, int B, int h, int wd, int Cout, void* stream);
+/* coords [B, h, w, 2] (x, y) = (init ? pixel grid : coords) + delta (planar [B, 2, h, w], may be NULL); flow_out (may be NULL) gets
+ * coords - grid at channel pitch flow_cpitch */
+int vt_raft_flow_f32(float* coords, const float* delta, int init, float* flow_out, int flow_cpitch, int B, int h, int w, void* stream);
+/* rh [npix, C] = sigmoid(zr[:, C:2C]) * h, zr [npix, 2C] = (z | r) logits */
+int vt_raft_gru_reset_f32(const float* zr, const float* h, float* rh, int64_t npix, int C, void* stream);
+/* h = (1 - z) * h + z * tanh(q), z = sigmoid(zr[:, :C]), in place */
+int vt_raft_gru_update_f32(const float* zr, const float* q, float* h, int64_t npix, int C, void* stream);
+/* RAFT.upsample_flow: mask NHWC [B, h, w, mask_cpitch] (576 logits, already scaled), flow = coords - grid -> up planar [B, 2, 8h, 8w];
+ * flow_low (may be NULL) planar [B, 2, h, w] = the flow */
+int vt_raft_upsample_f32(const float* mask, int mask_cpitch, const float* coords, float* up, float* flow_low, int B, int h, int w,
+                         void* stream);
+
 /* ---- elementwise helpers ------------------------------------------------------------------ */
 /* out = a * scale_a + b * scale_b (b may be NULL) */
 int vt_axpby_f32(const float* a, const float* b, float* out, int64_t n, float scale_a, float scale_b, int round_tf32, void* stream);

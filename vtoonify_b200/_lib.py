@@ -115,6 +115,16 @@ SYMBOLS = {
     "vt_lpips_head_grad_nhwc": (c_int, [_P, _P, _P, c_int, c_int64, c_int, _P, _P, _P]),
     "vt_augment_affine_plan": (c_int, [_P, c_int, c_int, c_int, POINTER(c_int)]),
     "vt_augment_affine_f32": (c_int, [_P, _P, _P, _P] + [c_int] * 11 + [_P]),
+    "vt_raft_input_s2d_f32": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    "vt_raft_norm_relu_nhwc": (c_int, [_P, _P, _P, _P, _P, c_int, c_int64, c_int, _P]),
+    "vt_raft_context_f32": (c_int, [_P, _P, _P, c_int64, c_int, c_int, _P]),
+    "vt_raft_corr_pool_f32": (c_int, [_P, _P, c_int64, c_int, c_int, c_int64, _P]),
+    "vt_raft_corr_lookup_f32": (c_int, [POINTER(c_void_p), POINTER(c_int64), c_int, c_int, _P, _P, c_int, c_int64, _P]),
+    "vt_raft_convf1_f32": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    "vt_raft_flow_f32": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P]),
+    "vt_raft_gru_reset_f32": (c_int, [_P, _P, _P, c_int64, c_int, _P]),
+    "vt_raft_gru_update_f32": (c_int, [_P, _P, _P, c_int64, c_int, _P]),
+    "vt_raft_upsample_f32": (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, _P]),
     "vt_resize_nearest_nhwc_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "vt_logits_readout_f32": (c_int, [_P, _P] + [c_int] * 10 + [c_float, c_int64, _P]),
     "vt_adain_affine_f32": (c_int, [_P, _P, _P, c_int, c_int, _P]),

@@ -448,6 +448,17 @@ int vt_raft_gru_update_f32(const float* zr, const float* q, float* h, int64_t np
 int vt_raft_upsample_f32(const float* mask, int mask_cpitch, const float* coords, float* up, float* flow_low, int B, int h, int w,
                          void* stream);
 
+/* ---- parsing-map smoothing (smooth_parsing_map.py warp and window fusion; vtoonify_b200.smooth_parsing) ---- */
+/* the script's warp(x, flo): out [B, C, H, W] = grid_sample(x, grid + flow, align_corners=True, zeros) * mask and mask (may be NULL)
+ * [B, C, H, W] = the sampled ones thresholded (< 0.9999 -> 0, then > 0 -> 1); flow planar [B, 2, H, W] in pixels (x, y) */
+int vt_flow_warp_f32(const float* x, const float* flow, float* out, float* mask, int B, int C, int H, int W, void* stream);
+/* one centre frame of the window fusion: nslot = 2 * window + 1 (at most 63) slots, host arrays of device pointers img[k] [3, H, W],
+ * par[k] [C, H, W], flow[k] [2, H, W] (flow[window] is not read) and host temporal weights wt[k]; out [C, H, W] = sum_k par'_k * w_k /
+ * sum_k w_k, with w_k = wt[k] * exp(-mean_c((I'_k - I_window)^2) / 0.08) * mask_k for the warped (') neighbours and w = wt[window] with
+ * the unwarped par[window] at the centre */
+int vt_parsing_fuse_f32(const float* const* img, const float* const* par, const float* const* flow, const float* wt, int nslot,
+                        float* out, int C, int H, int W, void* stream);
+
 /* ---- elementwise helpers ------------------------------------------------------------------ */
 /* out = a * scale_a + b * scale_b (b may be NULL) */
 int vt_axpby_f32(const float* a, const float* b, float* out, int64_t n, float scale_a, float scale_b, int round_tf32, void* stream);

@@ -6,7 +6,7 @@ OUT="$HERE/../lib"
 mkdir -p "$OUT"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall --expt-relaxed-constexpr"
-SRCS="api.cu upfirdn2d.cu elementwise.cu modulate.cu conv_direct.cu norm_fir.cu resample.cu frame_prep.cu conv_tc.cu conv_rs.cu conv_wgrad.cu lpips.cu augment.cu raft.cu"
+SRCS="api.cu upfirdn2d.cu elementwise.cu modulate.cu conv_direct.cu norm_fir.cu resample.cu frame_prep.cu conv_tc.cu conv_rs.cu conv_wgrad.cu lpips.cu augment.cu raft.cu smooth.cu"
 OBJS=""
 pids=()
 for s in $SRCS; do

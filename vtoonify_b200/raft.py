@@ -293,6 +293,16 @@ class RAFT(nn.Module):
         return _conv([x], self._plain(name + ".out", enc.conv2, x.shape[3]), ops.conv_taps(1, 0))
 
     # ------------------------------------------------------------------------------------------ forward
+    def _check_model(self):
+        """the module-level limits of the forward: eval mode, and no parameter that requires grad in grad mode"""
+        if self.training:
+            raise NotImplementedError("RAFT: train mode is not supported (BatchNorm would need batch statistics); call .eval()")
+        if torch.is_grad_enabled():
+            for nm, p in self.named_parameters():
+                if p.requires_grad:
+                    raise NotImplementedError(f"RAFT: parameter {nm} requires grad; the module is forward only "
+                                              "(run it under torch.no_grad())")
+
     def _check(self, image1, image2, iters, flow_init):
         if self.training:
             raise NotImplementedError("RAFT: train mode is not supported (BatchNorm would need batch statistics); call .eval()")
@@ -321,23 +331,47 @@ class RAFT(nn.Module):
             return self._forward(image1.contiguous(), image2.contiguous(), int(iters), flow_init, test_mode)
 
     def _forward(self, image1, image2, iters, flow_init, test_mode):
-        lib, st = load(), ops._stream()
+        B = image1.shape[0]
+        with ops.nvtx_range("raft.encoders"):
+            z = self._input_s2d(image1, image2)
+            fmap = self._features(z)                                   # [2B, h, w, 256]: fmap1 | fmap2
+            net, x = self._context(z[:B])
+        return self._iterate(fmap[:B], fmap[B:], net, x, iters, flow_init, test_mode)
+
+    # the three steps of the forward, also used on their own by smooth_parsing.smooth_parsing_maps, which encodes each frame once
+    def _input_s2d(self, image1, image2=None):
+        """the space-to-depth stem input [n, H/2, W/2, 32] of 2 * (x / 255) - 1 for image1 (then image2), planar [B, 3, H, W] in 0..255"""
         B, _, H, W = image1.shape
-        h, w = H // 8, W // 8
-        dev = image1.device
+        z = torch.empty(((1 if image2 is None else 2) * B, H // 2, W // 2, 32), device=image1.device, dtype=torch.float32)
+        check(load().vt_raft_input_s2d_f32(image1.data_ptr(), ops._ptr(image2), z.data_ptr(), B, H, W, 32, ops._stream()))
+        return z
+
+    def _features(self, z):
+        """the encoder step: fnet's features NHWC [n, H/8, W/8, 256] of the stem inputs z (instance norm: per sample)"""
+        return self._encode("fnet", self.fnet, z)
+
+    def _context(self, z):
+        """the context step: cnet on the stem inputs z -> the GRU state net [n, h, w, 128] = tanh and the GRU input buffer
+        x [n, h, w, 256] whose channels 0..127 hold inp = relu (the iterations write the rest)"""
+        n, H2, W2, _ = z.shape
+        h, w = H2 // 4, W2 // 4
+        cnet = self._encode("cnet", self.cnet, z)                     # [n, h, w, 256]
+        net = torch.empty((n, h, w, HDIM), device=z.device, dtype=torch.float32)
+        x = torch.empty((n, h, w, 256), device=z.device, dtype=torch.float32)      # GRU input [inp | motion | flow]
+        check(load().vt_raft_context_f32(cnet.data_ptr(), net.data_ptr(), x.data_ptr(), n * h * w, HDIM, 256, ops._stream()))
+        return net, x
+
+    def _iterate(self, fmap1, fmap2, net, x, iters, flow_init=None, test_mode=True):
+        """the iteration step: correlation pyramid of (fmap1, fmap2) [B, h, w, 256], ``iters`` updates of the GRU state ``net`` and
+        input ``x`` (both updated in place), mask head and convex up-sampling; returns what ``forward`` returns"""
+        lib, st = load(), ops._stream()
+        B, h, w, _ = fmap1.shape
+        H, W = 8 * h, 8 * w
+        dev = fmap1.device
         ub = self.update_block
 
-        with ops.nvtx_range("raft.encoders"):
-            z = torch.empty((2 * B, H // 2, W // 2, 32), device=dev, dtype=torch.float32)
-            check(lib.vt_raft_input_s2d_f32(image1.data_ptr(), image2.data_ptr(), z.data_ptr(), B, H, W, 32, st))
-            fmap = self._encode("fnet", self.fnet, z)                  # [2B, h, w, 256]: fmap1 | fmap2
-            cnet = self._encode("cnet", self.cnet, z[:B])              # [B, h, w, 256]
-            net = torch.empty((B, h, w, HDIM), device=dev, dtype=torch.float32)
-            x = torch.empty((B, h, w, 256), device=dev, dtype=torch.float32)      # GRU input [inp | motion | flow]
-            check(lib.vt_raft_context_f32(cnet.data_ptr(), net.data_ptr(), x.data_ptr(), B * h * w, HDIM, 256, st))
-
         with ops.nvtx_range("raft.correlation"):
-            levels = self._pyramid(fmap, B, h, w)
+            levels = self._pyramid(fmap1, fmap2, B, h, w)
 
         coords = torch.empty((B, h, w, 2), device=dev, dtype=torch.float32)
         fi = None if flow_init is None else flow_init.contiguous()
@@ -400,19 +434,19 @@ class RAFT(nn.Module):
             return low, preds[-1]
         return preds
 
-    def _pyramid(self, fmap, B, h, w):
+    def _pyramid(self, fmap1, fmap2, B, h, w):
         """the correlation pyramid: [(tensor, row stride, h_l, w_l)] of the 4 levels, level 0 [B, h, w, pad32(h*w)]"""
         lib, st = load(), ops._stream()
         hw = h * w
         cp = ops._pad32(hw)
-        wc = torch.zeros((B, 1, cp, 256), device=fmap.device, dtype=torch.float32)
-        wc[:, 0, :hw].copy_(fmap[B:].reshape(B, hw, 256))
-        c0 = ops.conv2d_nhwc([fmap[:B]], wc, [(0, 0, 0)], 1, h, w, alpha=1.0 / 16.0)   # fmap1 . fmap2 / sqrt(256)
+        wc = torch.zeros((B, 1, cp, 256), device=fmap1.device, dtype=torch.float32)
+        wc[:, 0, :hw].copy_(fmap2.reshape(B, hw, 256))
+        c0 = ops.conv2d_nhwc([fmap1], wc, [(0, 0, 0)], 1, h, w, alpha=1.0 / 16.0)   # fmap1 . fmap2 / sqrt(256)
         levels = [(c0, cp, h, w)]
         N = B * hw
         for _ in range(3):
             src, stride, hl, wl = levels[-1]
-            out = torch.empty((N, (hl // 2) * (wl // 2)), device=fmap.device, dtype=torch.float32)
+            out = torch.empty((N, (hl // 2) * (wl // 2)), device=fmap1.device, dtype=torch.float32)
             check(lib.vt_raft_corr_pool_f32(src.data_ptr(), out.data_ptr(), N, hl, wl, stride, st))
             levels.append((out, (hl // 2) * (wl // 2), hl // 2, wl // 2))
         return levels

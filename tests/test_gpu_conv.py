@@ -14,6 +14,13 @@ def maxerr(a, b):
     return (a.double() - b.double()).abs().max().item()
 
 
+def set_knob(lib, key, value):
+    """vt_set_option for a key the library must know (it returns -1 for an unknown key and changes nothing) -> old value"""
+    old = lib.vt_set_option(key, value)
+    assert old != -1, f"vt_set_option: the library has no option {key.decode()!r}"
+    return old
+
+
 def tf32_exact(shape, g, scale=1.0):
     """values with <= 8 significant bits: exactly representable in TF32 (10-bit mantissa)"""
     return (torch.randint(-64, 65, shape, generator=g).float() / 32.0) * scale
@@ -70,7 +77,7 @@ def test_tc_vs_direct_exact_data(case, mode):
     b = torch.randn(Cout, generator=g)
     ops.set_precision("fp32")
     ref = _run(ops, x, w, b, k, stride, pad, dil, "fp32")
-    old = _lib.load().vt_set_option(b"tc_mode", mode)
+    old = set_knob(_lib.load(), b"tc_mode", mode)
     try:
         y = _run(ops, x, w, b, k, stride, pad, dil, "tf32")
     finally:
@@ -187,7 +194,7 @@ def test_tc_m_tiles_per_work_item(case, mt):
     b = torch.randn(Cout, generator=g)
     ops.set_precision("fp32")
     ref = _run(ops, x, w, b, k, stride, pad, dil, "fp32")
-    old = _lib.load().vt_set_option(b"tc_mt", mt)
+    old = set_knob(_lib.load(), b"tc_mt", mt)
     try:
         y = _run(ops, x, w, b, k, stride, pad, dil, "tf32")
     finally:
@@ -227,12 +234,12 @@ def test_folded_upconv(shape):
     assert maxerr(ops.to_nchw(t).cpu(), ref) <= 5e-3 * max(1.0, ref.abs().max().item())
 
 
-@pytest.mark.parametrize("cg2", [0, 1, 2])
+@pytest.mark.parametrize("mt", [0, 1, 2])
 @pytest.mark.parametrize("case", [CASES[1], CASES[2], CASES[3], CASES[4], CASES[5], (2, 256, 256, 40, 24, 3, 1, 1, 1), (1, 512, 512, 16, 16, 3, 1, 4, 4),
                                   (2, 64, 256, 17, 9, 3, 1, 1, 1), (2, 32, 32, 33, 70, 3, 1, 1, 1)])
-def test_tc_cta_pairs(case, cg2):
-    """The tensor-core kernel vs the FFMA kernel on Cout-256 layers (the "tc_cg2" key of the Blackwell CTA-pair build is unknown
-    to the Hopper library: every parameter set runs the single-CTA kernel)."""
+def test_tc_m_tiles_with_epilogue(case, mt):
+    """The tensor-core kernel vs the FFMA kernel on the Cout-256 layers and their neighbours, with the full epilogue (leaky ReLU,
+    gain, residual with alpha / beta), for the automatic, one and two M tiles per work item (tc_mt)."""
     from vtoonify_b200 import _lib, ops
     B, Cin, Cout, H, W, k, stride, pad, dil = case
     g = torch.Generator().manual_seed(hash(case) % 10007)
@@ -243,14 +250,14 @@ def test_tc_cta_pairs(case, cg2):
     ops.set_precision("fp32")
     kw = dict(act=_lib.ACT_LRELU, slope=0.2, gain=1.25, alpha=0.5, beta=0.75)
     ref = _run(ops, x, w, b, k, stride, pad, dil, "fp32", res=ops.to_nhwc(res.cuda(), round_tf32=False), **kw)
-    old = _lib.load().vt_set_option(b"tc_cg2", cg2)
+    old = set_knob(_lib.load(), b"tc_mt", mt)
     try:
         y = _run(ops, x, w, b, k, stride, pad, dil, "tf32", res=ops.to_nhwc(res.cuda(), round_tf32=False), **kw)
     finally:
-        _lib.load().vt_set_option(b"tc_cg2", old)
+        _lib.load().vt_set_option(b"tc_mt", old)
         ops.set_precision(ops.DEFAULT_PRECISION)
     scale = ref.abs().max().item()
-    assert maxerr(y, ref) <= 2e-5 * max(1.0, scale), f"cg2 {cg2}: err {maxerr(y, ref):.3e} (scale {scale:.1f})"
+    assert maxerr(y, ref) <= 2e-5 * max(1.0, scale), f"mt {mt}: err {maxerr(y, ref):.3e} (scale {scale:.1f})"
 
 
 # ---- bf16x3: split-operand tensor-core mode on arbitrary fp32 data ------------------------------------------------------
@@ -268,7 +275,7 @@ def test_bf16x3_vs_direct_random_data(case, mode):
     b = torch.randn(Cout, generator=g)
     ops.set_precision("fp32")
     ref = _run(ops, x, w, b, k, stride, pad, dil, "fp32")
-    old = _lib.load().vt_set_option(b"tc_mode", mode)
+    old = set_knob(_lib.load(), b"tc_mode", mode)
     try:
         y = _run(ops, x, w, b, k, stride, pad, dil, "bf16x3")
     finally:
@@ -280,9 +287,10 @@ def test_bf16x3_vs_direct_random_data(case, mode):
     assert err <= BF16X3_TOL * scale
 
 
-@pytest.mark.parametrize("mt,cg2", [(1, 0), (1, 1), (2, 0), (4, 0)])
+@pytest.mark.parametrize("mt,m_major", [(1, 0), (1, 1), (2, 0), (4, 0)])
 @pytest.mark.parametrize("case", [CASES[2], CASES[3], CASES[5], (2, 256, 256, 40, 24, 3, 1, 1, 1), (2, 64, 256, 17, 9, 3, 1, 1, 1)])
-def test_bf16x3_work_item_shapes(case, mt, cg2):
+def test_bf16x3_work_item_shapes(case, mt, m_major):
+    """M tiles per work item (tc_mt) and work-item order (tc_m_major: the N tiles of a pixel tile side by side, or N-tile-major)"""
     from vtoonify_b200 import _lib, ops
     B, Cin, Cout, H, W, k, stride, pad, dil = case
     g = torch.Generator().manual_seed(hash(case) % 10007 + 2)
@@ -294,14 +302,14 @@ def test_bf16x3_work_item_shapes(case, mt, cg2):
     ops.set_precision("fp32")
     ref = _run(ops, x, w, b, k, stride, pad, dil, "fp32", res=ops.to_nhwc(res.cuda(), round_tf32=False), **kw)
     lib = _lib.load()
-    old = (lib.vt_set_option(b"tc_mt", mt), lib.vt_set_option(b"tc_cg2", cg2))
+    old = (set_knob(lib, b"tc_mt", mt), set_knob(lib, b"tc_m_major", m_major))
     try:
         y = _run(ops, x, w, b, k, stride, pad, dil, "bf16x3", res=ops.to_nhwc(res.cuda(), round_tf32=False), **kw)
     finally:
-        lib.vt_set_option(b"tc_mt", old[0]); lib.vt_set_option(b"tc_cg2", old[1])
+        lib.vt_set_option(b"tc_mt", old[0]); lib.vt_set_option(b"tc_m_major", old[1])
         ops.set_precision(ops.DEFAULT_PRECISION)
     scale = max(1.0, ref.abs().max().item())
-    assert maxerr(y, ref) <= BF16X3_TOL * scale, f"mt {mt} cg2 {cg2}: {maxerr(y, ref):.3e} (scale {scale:.1f})"
+    assert maxerr(y, ref) <= BF16X3_TOL * scale, f"mt {mt} m_major {m_major}: {maxerr(y, ref):.3e} (scale {scale:.1f})"
 
 
 @pytest.mark.parametrize("shape", [(2, 64, 32, 7, 9), (1, 128, 64, 16, 24), (1, 512, 256, 8, 8)])
@@ -332,12 +340,12 @@ def test_bf16x3_folded_upconv_and_concat(shape):
         ops.set_precision(ops.DEFAULT_PRECISION)
 
 
-@pytest.mark.parametrize("transpose,pair_y", [(0, 0), (0, 1), (2, 0), (2, 1)])
+@pytest.mark.parametrize("transpose,m_major", [(0, 0), (0, 1), (2, 0), (2, 1)])
 @pytest.mark.parametrize("case", [CASES[2], CASES[3], CASES[4], CASES[5], (2, 32, 32, 33, 20, 3, 1, 1, 1), (1, 64, 64, 9, 40, 1, 1, 0, 1),
                                   (1, 512, 512, 24, 16, 3, 1, 1, 1)])
-def test_tc_transposed_view_and_pair_orientation(case, transpose, pair_y):
+def test_tc_transposed_view_and_item_order(case, transpose, m_major):
     """The planner may hand the problem to the kernel transposed (x <-> y), a pure re-indexing that must not change results (noise,
-    residual and bias exercise every strided epilogue read); "tc_pair_y" is a key of the Blackwell CTA-pair build, ignored here."""
+    residual and bias exercise every strided epilogue read), in either work-item order (tc_m_major)."""
     from vtoonify_b200 import _lib, ops
     B, Cin, Cout, H, W, k, stride, pad, dil = case
     g = torch.Generator().manual_seed(hash(case) % 10007 + 5)
@@ -350,14 +358,14 @@ def test_tc_transposed_view_and_pair_orientation(case, transpose, pair_y):
     ops.set_precision("fp32")
     ref = _run(ops, x, w, b, k, stride, pad, dil, "fp32", res=ops.to_nhwc(res.cuda(), round_tf32=False), **kw)
     lib = _lib.load()
-    old = (lib.vt_set_option(b"tc_transpose", transpose), lib.vt_set_option(b"tc_pair_y", pair_y))
+    old = (set_knob(lib, b"tc_transpose", transpose), set_knob(lib, b"tc_m_major", m_major))
     try:
         y = _run(ops, x, w, b, k, stride, pad, dil, "bf16x3", res=ops.to_nhwc(res.cuda(), round_tf32=False), **kw)
     finally:
-        lib.vt_set_option(b"tc_transpose", old[0]); lib.vt_set_option(b"tc_pair_y", old[1])
+        lib.vt_set_option(b"tc_transpose", old[0]); lib.vt_set_option(b"tc_m_major", old[1])
         ops.set_precision(ops.DEFAULT_PRECISION)
     scale = max(1.0, ref.abs().max().item())
-    assert maxerr(y, ref) <= BF16X3_TOL * scale, f"T {transpose} pair_y {pair_y}: {maxerr(y, ref):.3e} (scale {scale:.1f})"
+    assert maxerr(y, ref) <= BF16X3_TOL * scale, f"T {transpose} m_major {m_major}: {maxerr(y, ref):.3e} (scale {scale:.1f})"
 
 
 @pytest.mark.parametrize("transpose", [0, 2])
@@ -374,7 +382,7 @@ def test_folded_upconv_transposed_view(shape, transpose):
     ref = O.upfirdn2d(F.conv_transpose2d(x, w.transpose(0, 1), stride=2), k4, pad=(1, 1))
     ref = F.leaky_relu(ref + nw * noise + bias.view(1, -1, 1, 1), 0.2) * 1.4142135
     lib = _lib.load()
-    old = lib.vt_set_option(b"tc_transpose", transpose)
+    old = set_knob(lib, b"tc_transpose", transpose)
     ops.set_precision("bf16x3")
     try:
         xn = ops.to_nhwc(x.cuda())
@@ -410,7 +418,7 @@ def test_smalln_input_stationary_vs_gather_kernel(shape, n_out):
     lib = _lib.load()
     outs = []
     for mode in (0, 2):
-        old = lib.vt_set_option(b"smalln_is", mode)
+        old = set_knob(lib, b"smalln_is", mode)
         try:
             y = ops.smalln_conv(xn, wp, ops.conv_taps(3, 1), n_out, B, H, W, planar=pl.cuda(), planar_weight=wpl, bias=b.cuda(),
                                 src2=x2n, tap_const=kc.cuda())
@@ -436,7 +444,7 @@ def test_bf16x3_second_source_scaled_per_pixel(case, transpose):
     b = torch.randn(Cout, generator=g)
     ref = F.conv2d(torch.cat([a, c * m], 1), w, b, padding=pad)
     lib = _lib.load()
-    old = lib.vt_set_option(b"tc_transpose", transpose)
+    old = set_knob(lib, b"tc_transpose", transpose)
     ops.set_precision("bf16x3")
     try:
         y = ops.conv2d_nhwc([ops.to_nhwc(a.cuda()), ops.to_nhwc(c.cuda())], ops.prep_weights(w.cuda(), cin_pad=C1 + 32),
@@ -463,7 +471,7 @@ def test_smalln_masked_source(mode):
     wp = ops.prep_weights(w[:, 3:].contiguous().cuda(), cin_pad=C)
     wpl = w[:, :3].permute(2, 3, 0, 1).reshape(9, 3, 3).contiguous().cuda()
     lib = _lib.load()
-    old = lib.vt_set_option(b"smalln_is", mode)
+    old = set_knob(lib, b"smalln_is", mode)
     try:
         y = ops.smalln_conv(ops.to_nhwc(x.cuda()), wp, ops.conv_taps(3, 1), 3, B, H, W, planar=pl.cuda(), planar_weight=wpl,
                             bias=b.cuda(), src_mask=m.cuda())
@@ -504,11 +512,12 @@ def test_smalln_conv_via_tensor_core_tap_products(with_planar, with_mask):
 
 
 @pytest.mark.parametrize("nstack", [False, True])
-@pytest.mark.parametrize("mt,cg2", [(0, 1), (1, 0), (2, 1), (4, 0)])
+@pytest.mark.parametrize("mt,m_major", [(0, 1), (1, 0), (2, 1), (4, 0)])
 @pytest.mark.parametrize("case", [CASES[0], CASES[2], CASES[9], (2, 32, 32, 33, 70, 3, 1, 1, 1), (1, 128, 32, 24, 40, 3, 1, 2, 2)])
-def test_bf16x3_n_stacked_weights(case, mt, cg2, nstack):
+def test_bf16x3_n_stacked_weights(case, mt, m_major, nstack):
     """Cout == 32: weight rows stacked as [w_hi|w_hi] x32 + [w_lo|w_lo] x32 (N = 64, 4 MMAs per tap, halves summed in the
-    epilogue) vs the 6-instruction form vs the FFMA kernel; with noise / bias / residual."""
+    epilogue) vs the 6-instruction form vs the FFMA kernel; with noise / bias / residual, M tiles per work item and work-item
+    order."""
     from vtoonify_b200 import _lib, ops
     B, Cin, Cout, H, W, k, stride, pad, dil = case
     g = torch.Generator().manual_seed(hash(case) % 10007 + 31)
@@ -521,27 +530,27 @@ def test_bf16x3_n_stacked_weights(case, mt, cg2, nstack):
     ops.set_precision("fp32")
     ref = _run(ops, x, w, b, k, stride, pad, dil, "fp32", res=ops.to_nhwc(res.cuda(), round_tf32=False), **kw)
     lib = _lib.load()
-    old = (lib.vt_set_option(b"tc_mt", mt), lib.vt_set_option(b"tc_cg2", cg2))
+    old = (set_knob(lib, b"tc_mt", mt), set_knob(lib, b"tc_m_major", m_major))
     ops.set_option("bf16x3_nstack", nstack)
     try:
         y = _run(ops, x, w, b, k, stride, pad, dil, "bf16x3", res=ops.to_nhwc(res.cuda(), round_tf32=False), **kw)
     finally:
         ops.set_option("bf16x3_nstack", False)
-        lib.vt_set_option(b"tc_mt", old[0]); lib.vt_set_option(b"tc_cg2", old[1])
+        lib.vt_set_option(b"tc_mt", old[0]); lib.vt_set_option(b"tc_m_major", old[1])
         ops.set_precision(ops.DEFAULT_PRECISION)
     scale = max(1.0, ref.abs().max().item())
-    assert maxerr(y, ref) <= BF16X3_TOL * scale, f"nstack {nstack} mt {mt} cg2 {cg2}: {maxerr(y, ref):.3e} (scale {scale:.1f})"
+    assert maxerr(y, ref) <= BF16X3_TOL * scale, f"nstack {nstack} mt {mt} m_major {m_major}: {maxerr(y, ref):.3e} (scale {scale:.1f})"
 
 
 @pytest.mark.parametrize("transpose", [0, 2])
 @pytest.mark.parametrize("case", [CASES[2], CASES[3], CASES[7], (2, 32, 32, 33, 70, 3, 1, 1, 1), "up"])
 def test_tc_epilogue_direct_global_stores(case, transpose):
-    """Epilogue variant that writes each pixel's 128-byte channel run straight to global memory (no smem staging / TMA store):
-    partial tiles, strided phase views (folded up-conv), transposed view, residual + noise."""
+    """The epilogue writes each pixel's channel pairs straight from the accumulator registers to global memory: partial tiles,
+    strided phase views (folded up-conv), transposed view, residual + noise."""
     from vtoonify_b200 import _lib, ops
     from oracle import vt_oracle as O
     lib = _lib.load()
-    old = (lib.vt_set_option(b"tc_direct_store", 1), lib.vt_set_option(b"tc_transpose", transpose))
+    old = set_knob(lib, b"tc_transpose", transpose)
     ops.set_precision("bf16x3")
     try:
         g = torch.Generator().manual_seed(41)
@@ -566,7 +575,7 @@ def test_tc_epilogue_direct_global_stores(case, transpose):
             ref = F.conv2d(x, w, b, stride=stride, padding=pad, dilation=dil) * 0.5 + 0.75 * res
             y = _run(ops, x, w, b, k, stride, pad, dil, "bf16x3", res=ops.to_nhwc(res.cuda()), alpha=0.5, beta=0.75)
     finally:
-        lib.vt_set_option(b"tc_direct_store", old[0]); lib.vt_set_option(b"tc_transpose", old[1])
+        lib.vt_set_option(b"tc_transpose", old)
         ops.set_precision(ops.DEFAULT_PRECISION)
     assert maxerr(y, ref) <= BF16X3_TOL * max(1.0, ref.abs().max().item()), f"{maxerr(y, ref):.3e}"
 
@@ -586,7 +595,7 @@ def test_bf16x3_per_channel_affine_on_source(case, transpose):
     xn = x * aff[:, :, 0, None, None] + aff[:, :, 1, None, None]
     ref = F.conv2d(xn, w, b, padding=pad, dilation=dil)
     lib = _lib.load()
-    old = lib.vt_set_option(b"tc_transpose", transpose)
+    old = set_knob(lib, b"tc_transpose", transpose)
     ops.set_precision("bf16x3")
     try:
         y = ops.conv2d_nhwc([ops.to_nhwc(x.cuda())], ops.prep_weights(w.cuda(), cin_pad=Cin), ops.conv_taps(k, pad, dil), 1, H, W,
@@ -614,14 +623,14 @@ def test_adain_affine_table_vs_adain_apply():
 
 
 # ---- round-2b scheduling options: same results whichever way they are set ---------------------------------------------
-@pytest.mark.parametrize("opt,values", [(b"tc_warp_store", (0, 1)), (b"tc_stage_policy", (0, 1)), (b"tc_halo_pct", (50, 60, 100))])
+@pytest.mark.parametrize("opt,values", [(b"tc_tgroup", (0, 1, 48)), (b"tc_stage_policy", (0, 1)), (b"tc_halo_pct", (50, 60, 100))])
 @pytest.mark.parametrize("case", [(2, 512, 512, 24, 40, 3, 1, 4, 4),     # dilation 4: the big-halo stage plan
                                   (1, 256, 256, 33, 20, 3, 1, 2, 2),
                                   (2, 64, 128, 19, 45, 3, 1, 1, 1),      # partial tiles in both directions
                                   (1, 128, 32, 16, 24, 1, 1, 0, 1)])     # 1x1, small N
 def test_tc_scheduling_options_do_not_change_results(case, opt, values):
-    """Per-warp vs CTA-wide output stores, the pipeline-stage plan of big halo boxes and the halo-staging threshold only change
-    WHEN data moves, never what is summed in which order: bit-identical outputs (csrc/conv_tc.cu)."""
+    """Taps per weight box (automatic, one, a 48 KB budget), the pipeline-stage plan of big halo boxes and the halo-staging
+    threshold only change WHEN data moves, never what is summed in which order: bit-identical outputs (csrc/conv_tc.cu)."""
     from vtoonify_b200 import _lib, ops
     B, Cin, Cout, H, W, k, stride, pad, dil = case
     g = torch.Generator().manual_seed(hash(case) % 10007 + 5)
@@ -632,10 +641,10 @@ def test_tc_scheduling_options_do_not_change_results(case, opt, values):
     ops.set_precision("fp32")
     ref = _run(ops, x, w, b, k, stride, pad, dil, "fp32")
     outs = []
-    old = lib.vt_set_option(opt, values[0])
+    old = set_knob(lib, opt, values[0])
     try:
         for v in values:
-            lib.vt_set_option(opt, v)
+            set_knob(lib, opt, v)
             outs.append(_run(ops, x, w, b, k, stride, pad, dil, "bf16x3"))
     finally:
         lib.vt_set_option(opt, old)
@@ -656,7 +665,7 @@ def test_instnorm_chunk_plans_agree(shape):
     x2 = ops.to_nhwc(torch.randn((B, C, H, W), generator=g).cuda())
     lib = _lib.load()
     res = {}
-    old = lib.vt_set_option(b"instnorm_chunks", 0)
+    old = set_knob(lib, b"instnorm_chunks", 0)
     try:
         for plan in (0, 296, 7):
             lib.vt_set_option(b"instnorm_chunks", plan)
@@ -691,7 +700,7 @@ def test_tc_fused_output_statistics(case, m_major):
     b = torch.randn(Cout, generator=g).cuda()
     res = ops.to_nhwc(torch.randn((B, Cout, H, W), generator=g).cuda(), round_tf32=False)
     lib = _lib.load()
-    old = lib.vt_set_option(b"tc_m_major", m_major)
+    old = set_knob(lib, b"tc_m_major", m_major)
     ops.set_precision("bf16x3")
     try:
         kw = dict(bias=b, act=_lib.ACT_LRELU, slope=0.2, gain=1.0, res=res, alpha=0.7, beta=0.7)

@@ -1,6 +1,5 @@
 """Row-strip up-convolution entry point (ops.conv_up2_rs_nhwc: Blur o conv_transpose2d as one convolution over the 4 output
-phases) against the fp32 polyphase transposed conv + FIR pass and the folded route.  The "rsu_*" keys belong to the Blackwell
-row-strip kernel and are unknown to the sm_90a library."""
+phases) against the fp32 polyphase transposed conv + FIR pass and the folded route."""
 import pytest
 import torch
 
@@ -14,14 +13,12 @@ def knobs():
     lib = _lib.load()
     old = {k: ops.get_option(k) for k in ("rs_min_width", "rs_fmt", "rsu_conv")}
     ops.set_option("rs_min_width", 1)
-    old_epi = lib.vt_set_option(b"rsu_epi", 1)
-    lib.vt_set_option(b"rsu_epi", old_epi)
+    old_t = lib.vt_set_option(b"tc_transpose", 1)
+    assert old_t != -1
     yield lib
     for k, v in old.items():
         ops.set_option(k, v)
-    lib.vt_set_option(b"rsu_cg", 0)
-    lib.vt_set_option(b"rsu_rows", 0)
-    lib.vt_set_option(b"rsu_epi", old_epi)
+    lib.vt_set_option(b"tc_transpose", old_t)
 
 
 def _blur():
@@ -43,27 +40,25 @@ def _case(B, Cin, Cout, H, W, wB, seed, noise):
 
 
 CASES = [
-    # B, Cin, Cout, H, W, wB, cg, rows_per_strip
-    (1, 64, 32, 12, 128, 1, 1, 0),
-    (1, 64, 32, 11, 100, 1, 1, 3),        # partial strip in x, several strips / ring laps in y
-    (2, 64, 32, 9, 260, 2, 2, 4),         # CTA pairs, per-sample weights
-    (1, 128, 64, 10, 140, 1, 1, 4),       # two output-channel passes, 4 K chunks
-    (2, 128, 64, 7, 300, 1, 2, 2),
-    (1, 32, 32, 5, 130, 1, 1, 1),         # one-row strips
-    (1, 64, 96, 6, 256, 1, 2, 0),         # three passes
+    # B, Cin, Cout, H, W, wB
+    (1, 64, 32, 12, 128, 1),
+    (1, 64, 32, 11, 100, 1),        # ragged in x and y
+    (2, 64, 32, 9, 260, 2),         # per-sample weights
+    (1, 128, 64, 10, 140, 1),       # N = 4 x 64 (two 128-wide N tiles, or one wide item), 4 K chunks
+    (2, 128, 64, 7, 300, 1),
+    (1, 32, 32, 5, 130, 1),
+    (1, 64, 96, 6, 256, 1),         # N = 4 x 96: 128-wide N tiles across phase boundaries
 ]
 
 
 @pytest.mark.parametrize("case", CASES, ids=[f"rsu{i}" for i in range(len(CASES))])
 @pytest.mark.parametrize("fmt,tol", [("bf16", 5e-5), ("f16", 6e-6)])
-@pytest.mark.parametrize("epi", [0, 1], ids=["epi0", "epi1"])   # one output row per pass / both rows per pass (csrc/conv_rsu.cu)
-def test_rsu_vs_fp32(knobs, case, fmt, tol, epi):
+@pytest.mark.parametrize("transpose", [0, 2], ids=["T0", "T2"])   # the kernel's view of the phase outputs as is / transposed (x <-> y)
+def test_rsu_vs_fp32(knobs, case, fmt, tol, transpose):
     from vtoonify_b200 import ops
-    B, Cin, Cout, H, W, wB, cg, rows = case
+    B, Cin, Cout, H, W, wB = case
     lib = knobs
-    lib.vt_set_option(b"rsu_epi", epi)
-    lib.vt_set_option(b"rsu_cg", cg)
-    lib.vt_set_option(b"rsu_rows", rows)
+    assert lib.vt_set_option(b"tc_transpose", transpose) != -1
     ops.set_option("rs_fmt", fmt)
     K = _blur()
     x, w9, kw = _case(B, Cin, Cout, H, W, wB, seed=B * 100 + H, noise=(H % 2 == 1))
@@ -74,7 +69,7 @@ def test_rsu_vs_fp32(knobs, case, fmt, tol, epi):
     assert tuple(y.shape) == (B, 2 * H, 2 * W, Cout)
     scale = ref.abs().max().item()
     err = (y - ref).abs().max().item()
-    print(f"conv_rsu {case} [{fmt}, epi {epi}]: max|err| {err:.3e} (max|ref| {scale:.2f})")
+    print(f"conv_rsu {case} [{fmt}, T {transpose}]: max|err| {err:.3e} (max|ref| {scale:.2f})")
     assert err <= tol * scale, f"{err:.3e} > {tol} * {scale:.2f}"
 
 

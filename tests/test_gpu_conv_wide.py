@@ -3,7 +3,11 @@
 Option tc_wide: 0 = 128-wide N tiles only, 1 = automatic (wide items on stride-1 layers, with the whole rounds wide and the
 last partial round as a second launch of 128-wide items), 2 = wide items in one launch, stride 2 included.  Each output element gets the same k16 products in the
 same order whatever the N tile, so all three must be bit-identical."""
+import json
+import os
 import re
+import subprocess
+import sys
 
 import numpy as np
 import pytest
@@ -188,9 +192,8 @@ def test_wide_remainder_split_writes_every_element(lib):
     assert_identical(outs)
 
 
-def test_wide_kernels_are_the_ones_that_run(lib):
-    """tc_wide 1 runs conv_tc_kernel<256, 1, 1> on the whole rounds and conv_tc_kernel<128, 1, 1> on the rest; 2 runs the
-    wide kernel alone; 0 the 128-wide kernel alone"""
+def traced_kernels(lib):
+    """{tc_wide mode: sorted conv_tc_kernel template arguments} of the split case, from torch.profiler traces"""
     from torch.profiler import ProfilerActivity, profile
     from vtoonify_b200 import ops
     B, Cin, Cout, H, W = _split_case(torch.cuda.get_device_properties(0).multi_processor_count)
@@ -208,7 +211,25 @@ def test_wide_kernels_are_the_ones_that_run(lib):
         names = [m.group(1) for e in prof.events() for m in [re.search(r"conv_tc_kernel<(\d+, \d+, \d+)>", e.name)] if m]
         return sorted(names)
 
-    got = per_mode(lib, kernels)
+    return per_mode(lib, kernels)
+
+
+def test_wide_kernels_are_the_ones_that_run():
+    """tc_wide 1 runs conv_tc_kernel<256, 1, 1> on the whole rounds and conv_tc_kernel<128, 1, 1> on the rest; 2 runs the
+    wide kernel alone; 0 the 128-wide kernel alone.  Traced in a child process whose only profiler sessions are these: traces
+    taken late in a long test process can come back without their kernels."""
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    args = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [os.path.abspath(__file__), "--trace-kernels"]
+    r = subprocess.run(args, cwd=root, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, f"kernel trace failed:\n{r.stdout[-2000:]}\n{r.stderr[-4000:]}"
+    line = [l for l in r.stdout.splitlines() if l.startswith("KERNELS ")][-1]
+    got = {int(k): v for k, v in json.loads(line[len("KERNELS "):]).items()}
     assert got[0] == ["128, 1, 1"]
     assert got[1] == ["128, 1, 1", "256, 1, 1"]
     assert got[2] == ["256, 1, 1"]
+
+
+if __name__ == "__main__" and sys.argv[1:] == ["--trace-kernels"]:
+    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    from vtoonify_b200 import _lib
+    print("KERNELS " + json.dumps(traced_kernels(_lib.load())))

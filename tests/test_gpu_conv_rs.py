@@ -1,21 +1,11 @@
-"""Row-strip entry point (vt_conv2d_rs: the full-resolution 3x3 layers with Cin, Cout in {32, 64}, including the image-only ToRGB
-launch) against the fp32 FFMA kernel and against the tap-by-tap tensor-core route on the same descriptors."""
+"""Row-strip entry point (vt_conv2d_rs: the full-resolution 3x3 layers with Cin, Cout in {32, 64}): the default routing by row
+width.  Every kernel instantiation, the fused ToRGB and the image-only launch are checked against float64 in
+test_gpu_conv_rs_plans.py."""
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
-
-
-@pytest.fixture()
-def rs_knobs():
-    from vtoonify_b200 import _lib, ops
-    lib = _lib.load()
-    old = {"rs_min_width": ops.get_option("rs_min_width"), "rs_fmt": ops.get_option("rs_fmt"), "rs_conv": ops.get_option("rs_conv")}
-    ops.set_option("rs_min_width", 1)
-    yield lib
-    for k, v in old.items():
-        ops.set_option(k, v)
 
 
 def _case(B, Cin, Cout, H, W, wB, seed, bias=True, noise=False, act=True):
@@ -31,74 +21,10 @@ def _case(B, Cin, Cout, H, W, wB, seed, bias=True, noise=False, act=True):
     return x, w, kw
 
 
-def _run(x, w, kw, H, W, rs, precision=None, rgb=None):
+def _run(x, w, kw, H, W, rs):
     from vtoonify_b200 import ops
     ops.set_option("rs_conv", rs)
-    return ops.conv2d_nhwc([x], w, ops.conv_taps(3, 1), 1, H, W, precision=precision, rgb=rgb, **kw)
-
-
-CASES = [
-    # B, Cin, Cout, H, W, wB
-    (1, 32, 32, 40, 128, 1),
-    (1, 32, 32, 37, 100, 1),        # ragged rows and columns
-    (2, 32, 32, 33, 300, 2),        # per-sample weights (weight reload between samples)
-    (2, 32, 32, 64, 256, 1),
-    (1, 64, 64, 30, 140, 1),        # two K chunks
-    (3, 64, 64, 21, 260, 3),
-    (1, 64, 32, 19, 130, 1),
-    (2, 32, 64, 23, 257, 2),
-]
-
-
-@pytest.mark.parametrize("case", CASES, ids=[f"rs{i}" for i in range(len(CASES))])
-@pytest.mark.parametrize("fmt,tol", [("bf16", 4e-5), ("f16", 4e-6)])
-def test_rs_vs_fp32(rs_knobs, case, fmt, tol):
-    from vtoonify_b200 import ops
-    B, Cin, Cout, H, W, wB = case
-    lib = rs_knobs
-    ops.set_option("rs_fmt", fmt)
-    x, w, kw = _case(B, Cin, Cout, H, W, wB, seed=B * 1000 + H, noise=(H % 2 == 1))
-    ref = _run(x, w, kw, H, W, rs=False, precision="fp32")
-    y = _run(x, w, kw, H, W, rs=True)
-    torch.cuda.synchronize()
-    scale = ref.abs().max().item()
-    err = (y - ref).abs().max().item()
-    print(f"conv_rs {case} [{fmt}]: max|err| {err:.3e} (max|ref| {scale:.2f})")
-    assert err <= tol * scale, f"{err:.3e} > {tol} * {scale:.2f}"
-    # the launch really went to the row-strip kernel
-    d_ok = lib.vt_conv2d_rs_supported
-    assert d_ok is not None
-
-
-@pytest.mark.parametrize("Cin,H,W,B,wB", [(32, 26, 128, 1, 1), (32, 40, 384, 2, 2), (64, 20, 256, 2, 1)])
-def test_rs_fused_torgb(rs_knobs, Cin, H, W, B, wB):
-    """fused ToRGB tail (1x1 modulated conv + bias + Upsample(skip)) of the row-strip epilogue == the tap-by-tap kernel's"""
-    from vtoonify_b200 import ops
-    x, w, kw = _case(B, Cin, Cin, H, W, wB, seed=5, noise=True)
-    g = torch.Generator().manual_seed(9)
-    k1 = torch.tensor([1., 3., 3., 1.])
-    rgb = {"w": (torch.randn((wB, 1, 3, Cin), generator=g) * 0.2).cuda(), "bias": (torch.randn(3, generator=g) * 0.1).cuda(),
-           "skip": torch.randn((B, 3, H // 2, W // 2), generator=g).cuda(), "kernel": (k1[:, None] * k1[None, :] / 64 * 4).cuda()}
-    ref, ref_rgb = _run(x, w, kw, H, W, rs=False, rgb=rgb)
-    y, y_rgb = _run(x, w, kw, H, W, rs=True, rgb=rgb)
-    torch.cuda.synchronize()
-    e1 = (y - ref).abs().max().item() / ref.abs().max().item()
-    e2 = (y_rgb - ref_rgb).abs().max().item() / ref_rgb.abs().max().item()
-    print(f"conv_rs + ToRGB Cin={Cin}: feature err {e1:.2e}, rgb err {e2:.2e}")
-    assert e1 <= 6e-5 and e2 <= 6e-5
-    # without skip
-    rgb2 = dict(rgb, skip=None, kernel=None)
-    _, r0 = _run(x, w, kw, H, W, rs=False, rgb=rgb2)
-    _, r1 = _run(x, w, kw, H, W, rs=True, rgb=rgb2)
-    assert (r0 - r1).abs().max().item() <= 6e-5 * r0.abs().max().item()
-    # RGB-only launch (the generator's last layer): no activation is written, the image is bit-identical; the tap-by-tap route
-    # ignores the hint and still returns the activation
-    for r in (rgb, rgb2):
-        none_out, only = _run(x, w, kw, H, W, rs=True, rgb=dict(r, only=True))
-        full_out, full = _run(x, w, kw, H, W, rs=True, rgb=r)
-        assert none_out is None and torch.equal(only, full)
-    o2, r2 = _run(x, w, kw, H, W, rs=False, rgb=dict(rgb, only=True))
-    assert o2 is not None and torch.equal(o2, ref) and torch.equal(r2, ref_rgb)
+    return ops.conv2d_nhwc([x], w, ops.conv_taps(3, 1), 1, H, W, **kw)
 
 
 def test_rs_default_routing():

@@ -32,7 +32,8 @@ def test_dataparallel_strict_load():
     dp = torch.nn.DataParallel(m)
     dp.load_state_dict(sd, strict=True)
     mod = dp.module
-    assert torch.equal(mod.cnet.layer2[0].norm3.running_var, sd["module.cnet.layer2.0.downsample.1.running_var"])
+    # (DataParallel moves the module to cuda:0 where a GPU exists)
+    assert torch.equal(mod.cnet.layer2[0].norm3.running_var.cpu(), sd["module.cnet.layer2.0.downsample.1.running_var"])
     assert mod.hidden_dim == 128 and mod.context_dim == 128
 
 

@@ -781,8 +781,11 @@ static int conv_tc_run(const vt_conv_desc* d, void* stream, int* chunks_out, int
     VT_CHECK(d->out_sb % d->out_cpitch == 0 && d->out_sy % d->out_cpitch == 0 && d->out_sx % d->out_cpitch == 0,
              "conv_tc: output strides must be multiples of out_cpitch when noise is used");
     a.pix_sb = d->out_sb / d->out_cpitch; a.pix_sy = g_out_sy / d->out_cpitch; a.pix_sx = g_out_sx / d->out_cpitch;
+    // a view's noise pixel is its element offset over out_cpitch (as in the FFMA kernel): the remainder is the channel offset
+    // of a channel slice, which has to keep the slice inside one pixel
     for (int ph = 0; ph < 4; ++ph) {
-      VT_CHECK(a.phase_off[ph] % d->out_cpitch == 0, "conv_tc: phase offset must be a multiple of out_cpitch");
+      VT_CHECK(a.phase_off[ph] >= 0 && a.phase_off[ph] % d->out_cpitch + d->Cout <= d->out_cpitch,
+               "conv_tc: with noise, the output view's channels must lie inside one pixel of out_cpitch channels");
       a.phase_pix[ph] = a.phase_off[ph] / d->out_cpitch;
     }
   }

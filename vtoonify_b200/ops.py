@@ -473,8 +473,21 @@ def conv2d_nhwc(srcs: Sequence[torch.Tensor], weight: torch.Tensor, taps, stride
     d.round_tf32 = _round_flag()
     rgb_out = None
     if rgb is not None:
-        # fused ToRGB tail: rgb = {"w": [wB,3,Cout], "bias": [3], "skip": [B,3,Ho/2,Wo/2] or None, "kernel": [4,4]}
+        # fused ToRGB tail: rgb = {"w": [wB,3,Cout] or [wB,1,3,Cout], "bias": [3], "skip": [B,3,Ho/2,Wo/2] or None, "kernel": [4,4]}
+        # with wB the conv weight's: the kernels read them by raw pointer, "w" as a dense [wB][3][Cout]
         _req_cuda(rgb["w"], rgb["bias"], rgb.get("skip"), rgb.get("kernel"))
+        rw, rb, skip, kern = rgb["w"], rgb["bias"], rgb.get("skip"), rgb.get("kernel")
+        if tuple(rw.shape) not in ((wB, 3, Cout), (wB, 1, 3, Cout)) or not rw.is_contiguous() or rw.dtype != torch.float32:
+            raise _lib.VtError(f"conv2d_nhwc: rgb['w'] must be a contiguous float32 [wB, 3, Cout] = [{wB}, 3, {Cout}] tensor "
+                               f"(got {rw.dtype} {tuple(rw.shape)}{'' if rw.is_contiguous() else ', not contiguous'})")
+        if rb.numel() != 3 or not rb.is_contiguous() or rb.dtype != torch.float32:
+            raise _lib.VtError("conv2d_nhwc: rgb['bias'] must be a contiguous float32 tensor of 3 elements")
+        if skip is not None:
+            if tuple(skip.shape) != (B, 3, Ho // 2, Wo // 2) or 2 * (Ho // 2) != Ho or 2 * (Wo // 2) != Wo or skip.dtype != torch.float32:
+                raise _lib.VtError(f"conv2d_nhwc: rgb['skip'] must be a float32 [B, 3, Ho/2, Wo/2] = [{B}, 3, {Ho / 2:g}, {Wo / 2:g}] "
+                                   f"tensor (got {tuple(skip.shape)})")
+            if kern is None or tuple(kern.shape) != (4, 4) or kern.dtype != torch.float32:
+                raise _lib.VtError("conv2d_nhwc: rgb['kernel'] must be a float32 4x4 up-sampling kernel when rgb['skip'] is given")
         rgb_out = torch.empty((B, 3, Ho, Wo), device=srcs[0].device, dtype=torch.float32)
         d.rgb_w, d.rgb_bias, d.rgb_out = rgb["w"].data_ptr(), rgb["bias"].data_ptr(), rgb_out.data_ptr()
         if rgb.get("skip") is not None:

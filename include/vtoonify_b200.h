@@ -458,6 +458,17 @@ int vt_flow_warp_f32(const float* x, const float* flow, float* out, float* mask,
  * the unwarped par[window] at the centre */
 int vt_parsing_fuse_f32(const float* const* img, const float* const* par, const float* const* flow, const float* wt, int nslot,
                         float* out, int C, int H, int W, void* stream);
+/* B centres of the window fusion, each followed by Downsample([1, 3, 3, 1], 2) and a scale: img / par / flow are host arrays of
+ * B * nslot device pointers (centre b's slot k at b * nslot + k, as for vt_parsing_fuse_f32); out + b * out_bstride [C, H / 2, W / 2]
+ * (contiguous per sample) = scale * down(fuse_b), TF32-rounded when round_tf32.  Bit-identical to vt_parsing_fuse_f32, then
+ * vt_upfirdn2d_f32 (kernel outer([1,3,3,1]) / 64, down 2, pad 1), then vt_axpby_f32 with the same scale and rounding; the fused map is
+ * never written to memory */
+int vt_parsing_fuse_down_f32(const float* const* img, const float* const* par, const float* const* flow, const float* wt, int nslot,
+                             int B, float* out, int64_t out_bstride, int C, int H, int W, float scale, int round_tf32, void* stream);
+/* the frame prep of smoothing from uint8 RGB frames [B, H, W, 3]: img planar [B, 3, 2H, 2W] = F.interpolate(Normalize(ToTensor(frame)),
+ * scale_factor=2, mode='bilinear') (the up-sampling of vt_frame_s2d_f32, without its factor 2) and stem NHWC [B, H, W, cpad] = RAFT's
+ * space-to-depth stem input (vt_raft_input_s2d_f32) of (img + 1) * 255 / 2, rounded after the add, the multiply and the divide */
+int vt_smooth_frame_prep_u8(const uint8_t* frames, float* img, float* stem, int B, int H, int W, int cpad, void* stream);
 
 /* ---- elementwise helpers ------------------------------------------------------------------ */
 /* out = a * scale_a + b * scale_b (b may be NULL) */

@@ -128,6 +128,9 @@ SYMBOLS = {
     "vt_flow_warp_f32": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     "vt_parsing_fuse_f32": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_float), c_int, _P, c_int, c_int,
                                     c_int, _P]),
+    "vt_parsing_fuse_down_f32": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_float), c_int, c_int, _P,
+                                         c_int64, c_int, c_int, c_int, c_float, c_int, _P]),
+    "vt_smooth_frame_prep_u8": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     "vt_resize_nearest_nhwc_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "vt_logits_readout_f32": (c_int, [_P, _P] + [c_int] * 10 + [c_float, c_int64, _P]),
     "vt_adain_affine_f32": (c_int, [_P, _P, _P, c_int, c_int, _P]),

@@ -46,6 +46,33 @@ __device__ __forceinline__ float vt_round_tf32(float x) {
 
 __device__ __forceinline__ float vt_lrelu(float v, float slope) { return v > 0.f ? v : v * slope; }
 
+// ToTensor + Normalize(0.5, 0.5) of one uint8 sample: v / 255, then (v - 0.5) / 0.5 (torchvision's order)
+__device__ __forceinline__ float vt_u8_unit(unsigned v) { return (((float)v / 255.f) - 0.5f) / 0.5f; }
+
+// RAFT's input normalisation 2 * (x / 255) - 1 of a sample in 0..255
+__device__ __forceinline__ float vt_raft_unit(float v) { return 2.f * (v / 255.f) - 1.f; }
+
+// F.interpolate(scale_factor=2, mode='bilinear', align_corners=False) of one [Hin, Win] plane at output pixel (Y, X); ld(offset) reads
+// the plane.  Every kernel that up-samples frames calls this one function, so they agree bit for bit.  The roundings are explicit:
+// left to the compiler, the contraction of w0*a + w1*b into an fma depends on the surrounding code (whether a product has other
+// uses), and two kernels inlining the same expression computed different bits.  The fmas below are the ones frame_s2d_kernel was
+// compiled to before this function existed (the sum h0*(w0*a + w1*b) + h1*(w0*c + w1*d) of ATen's upsample_bilinear2d).
+template <class Load>
+__device__ __forceinline__ float vt_bilinear_up2(Load ld, int Y, int X, int Hin, int Win) {
+  // src = (dst + 0.5) / 2 - 0.5, clamped at 0 (the multiply by 0.5 is exact, so the fma rounds once like the expression)
+  float sy = fmaf(__fadd_rn((float)Y, 0.5f), 0.5f, -0.5f), sx = fmaf(__fadd_rn((float)X, 0.5f), 0.5f, -0.5f);
+  sy = sy < 0.f ? 0.f : sy; sx = sx < 0.f ? 0.f : sx;
+  const int y0 = (int)sy, x0 = (int)sx;
+  const int y1 = y0 + (y0 < Hin - 1 ? 1 : 0), x1 = x0 + (x0 < Win - 1 ? 1 : 0);
+  const float ly = __fsub_rn(sy, (float)y0), lx = __fsub_rn(sx, (float)x0);
+  const float hy = __fsub_rn(1.f, ly), hx = __fsub_rn(1.f, lx);
+  const float a = ld((int64_t)y0 * Win + x0), bq = ld((int64_t)y0 * Win + x1);
+  const float cq = ld((int64_t)y1 * Win + x0), d = ld((int64_t)y1 * Win + x1);
+  const float top = fmaf(lx, bq, __fmul_rn(hx, a));
+  const float bot = fmaf(hx, cq, __fmul_rn(lx, d));
+  return fmaf(hy, top, __fmul_rn(ly, bot));
+}
+
 // Rank-1 test of a (flipped) 4x4 FIR kernel held in shared memory: k = ay (x) bx, with bx normalised by the smallest non-zero entry of
 // the pivot row so that integer-ratio filters (outer([1,3,3,1]), every StyleGAN blur) factor exactly.  Returns false for a full-rank
 // kernel (the caller then applies the 16 taps directly).

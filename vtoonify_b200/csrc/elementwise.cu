@@ -103,9 +103,9 @@ frame_u8_to_f32_kernel(const uint8_t* __restrict__ in, float* __restrict__ out, 
     uint8_t c0 = ip[p * 3 + 0], c1 = ip[p * 3 + 1], c2 = ip[p * 3 + 2];
     if (swap_rb) { uint8_t t = c0; c0 = c2; c2 = t; }
     // ToTensor: v/255 ; Normalize(0.5, 0.5): (v - 0.5) / 0.5   (same op order as torchvision)
-    op[p] = (((float)c0 / 255.f) - 0.5f) / 0.5f;
-    op[HW + p] = (((float)c1 / 255.f) - 0.5f) / 0.5f;
-    op[2 * HW + p] = (((float)c2 / 255.f) - 0.5f) / 0.5f;
+    op[p] = vt_u8_unit(c0);
+    op[HW + p] = vt_u8_unit(c1);
+    op[2 * HW + p] = vt_u8_unit(c2);
   }
 }
 

@@ -44,7 +44,7 @@ raft_input_s2d_kernel(const float* __restrict__ img1, const float* __restrict__ 
     for (int q = 0; q < 4; ++q) {
       const int Y = 2 * y + (q >> 1), X = 2 * x + (q & 1);
 #pragma unroll
-      for (int c = 0; c < 3; ++c) op[q * 3 + c] = 2.f * (__ldg(ip + ((int64_t)c * H + Y) * W + X) / 255.f) - 1.f;
+      for (int c = 0; c < 3; ++c) op[q * 3 + c] = vt_raft_unit(__ldg(ip + ((int64_t)c * H + Y) * W + X));
     }
     for (int c = 12; c < cpad; ++c) op[c] = 0.f;
   }

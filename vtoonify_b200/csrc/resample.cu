@@ -28,16 +28,9 @@ frame_s2d_kernel(const float* __restrict__ in, float* __restrict__ out, int Hin,
           if (mode == 0) {
             r = __ldg(pl + (int64_t)Y * Win + X);
           } else {
-            // F.interpolate(scale_factor=2, mode='bilinear', align_corners=False): src = (dst + 0.5) / 2 - 0.5, clamped at 0
-            float sy = (Y + 0.5f) * 0.5f - 0.5f, sx = (X + 0.5f) * 0.5f - 0.5f;
-            sy = sy < 0.f ? 0.f : sy; sx = sx < 0.f ? 0.f : sx;
-            const int y0 = (int)sy, x0 = (int)sx;
-            const int y1 = y0 + (y0 < Hin - 1 ? 1 : 0), x1 = x0 + (x0 < Win - 1 ? 1 : 0);
-            const float ly = sy - (float)y0, lx = sx - (float)x0;
-            const float a = __ldg(pl + (int64_t)y0 * Win + x0), bq = __ldg(pl + (int64_t)y0 * Win + x1);
-            const float cq = __ldg(pl + (int64_t)y1 * Win + x0), d = __ldg(pl + (int64_t)y1 * Win + x1);
-            // same association as ATen's upsample_bilinear2d: h0*(w0*a + w1*b) + h1*(w0*c + w1*d)
-            r = 2.f * ((1.f - ly) * ((1.f - lx) * a + lx * bq) + ly * ((1.f - lx) * cq + lx * d));
+            // 2 * F.interpolate(scale_factor=2, mode='bilinear', align_corners=False); the frame prep of smoothing
+            // (vt_smooth_frame_prep_u8) writes the same up-sampling without the factor 2
+            r = 2.f * vt_bilinear_up2([&](int64_t o) { return __ldg(pl + o); }, Y, X, Hin, Win);
           }
         }
         v[q * 3 + c] = r;

@@ -16,6 +16,7 @@ the clip, every round it scatters one input batch per rank and gathers the uint8
 (NCCL on NVLink for CUDA tensors, gloo in the CPU tests), overlapped with the synthesis of the neighbouring rounds.
 :func:`scatter_batches` / :func:`gather_frames` are the same collectives in their simple blocking form.
 """
+import collections
 import contextlib
 from typing import Callable, Iterable, Iterator, List, Optional, Sequence
 
@@ -23,6 +24,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops
+from . import smooth_parsing
 
 
 def shard_indices(num_batches: int, rank: int, world: int) -> List[int]:
@@ -45,6 +47,16 @@ class FramePipeline:
         the parsing maps are computed on the device (style_transfer.py:171-174); with ``prefilter`` the frames are the
         clip's full-resolution frames and the blur / resize / crop of style_transfer.py:151-156 also runs on the device.
 
+    Temporally smoothed parsing (``smoothing=(raft_model, window, iters)``, smooth_parsing_map.py followed by
+    ``style_transfer.py --parsing_map_path`` in one pass): batches are uint8 frames (``prefilter`` allowed) and ``parsing_net`` is
+    required.  Per input batch the frames are up-sampled 2x with RAFT's stem input (``smooth_parsing.frame_prep``), BiSeNet gives
+    the 2x logits (the script's ``parsingpredictor(2 * Is)``) and every frame is pushed into a ``smooth_parsing.ParsingSmoother``; each
+    output it releases is fused, down-sampled and scaled by 1/16 straight into its frame's network input
+    (``smooth_parsing.parsing_fuse_down``).  Output batch j holds the frames of input batch j: the first outputs wait ``window``
+    frames and the end of the input flushes the rest.  Device memory holds the window, not the clip; no intermediate file is
+    written.  H and W (after ``prefilter``) must be multiples of 8 and at least 64; ``graph`` is not supported (the launches of a
+    batch depend on where it sits in the clip).
+
     Buffer ownership.  With ``copy=True`` (default) every yielded tensor is a fresh host tensor owned by the caller.
     With ``copy=False`` the yielded tensor is a *borrowed* view of one of ``ring`` pinned staging buffers: it stays valid
     until ``ring - 1`` further batches have been yielded (``ring=3``: the previous result is still intact while the
@@ -54,9 +66,20 @@ class FramePipeline:
 
     def __init__(self, model, style: torch.Tensor, d_s: Optional[float] = 0.5, device: Optional[torch.device] = None,
                  output: str = "u8", parsing_net=None, ring: int = 3, copy: bool = True, graph: bool = False,
-                 prefilter=None):
+                 prefilter=None, smoothing=None):
         if ring < 2:
             raise ValueError("FramePipeline: ring must be >= 2 (one buffer is being filled while one is being consumed)")
+        if smoothing is not None:
+            if graph:
+                raise ValueError("FramePipeline: graph=True is not supported with smoothing (a batch's launches depend on its place "
+                                 "in the clip)")
+            if parsing_net is None:
+                raise ValueError("FramePipeline: smoothing needs parsing_net (the 2x parsing logits are computed on the device)")
+            raft_model, window, iters = smoothing
+            with torch.no_grad():           # the run is forward only
+                smooth_parsing._check_model_window("FramePipeline", raft_model, window, iters)
+            smoothing = (raft_model, int(window), int(iters))
+        self.smoothing = smoothing
         self.model = model
         self.device = device or next(model.parameters()).device
         self.style = style.to(self.device)
@@ -167,21 +190,12 @@ class FramePipeline:
         return self._host_out[key]
 
     def run(self, batches: Iterable) -> Iterator[torch.Tensor]:
+        compute = self._compute_smoothed(batches) if self.smoothing is not None else self._compute(batches)
         main = torch.cuda.current_stream(self.device)
-        it = iter(batches)
-        nxt = next(it, None)
         pending = None  # (host_tensor, event) of the previous batch's download
         slot = 0
-        up = self._upload(nxt) if nxt is not None else None
         with torch.no_grad():
-            while up is not None:
-                x, ev = up
-                nxt = next(it, None)
-                up = self._upload(nxt) if nxt is not None else None   # prefetch the next batch while this one computes
-                main.wait_event(ev)
-                for t in (x if isinstance(x, tuple) else (x,)):
-                    t.record_stream(main)
-                out_dev = self.process(x)
+            for out_dev in compute:
                 done = torch.cuda.Event()
                 done.record(main)
                 host = self._host_buffer(out_dev.shape, out_dev.dtype, slot)
@@ -200,6 +214,79 @@ class FramePipeline:
             if pending is not None:
                 pending[1].synchronize()
                 yield pending[0].clone() if self.copy else pending[0]
+
+    def _uploaded(self, batches: Iterable):
+        """the device items of ``batches`` in order, each made ready on the current stream; the next batch's upload is issued before
+        the current one is handed out, so it overlaps the current batch's compute"""
+        main = torch.cuda.current_stream(self.device)
+        it = iter(batches)
+        nxt = next(it, None)
+        up = self._upload(nxt) if nxt is not None else None
+        while up is not None:
+            x, ev = up
+            nxt = next(it, None)
+            up = self._upload(nxt) if nxt is not None else None   # prefetch the next batch while this one computes
+            main.wait_event(ev)
+            for t in (x if isinstance(x, tuple) else (x,)):
+                t.record_stream(main)
+            yield x
+
+    def _compute(self, batches: Iterable):
+        """one device result per input batch"""
+        for x in self._uploaded(batches):
+            yield self.process(x)
+
+    def _compute_smoothed(self, batches: Iterable):
+        """one device result per input batch through the streaming smoother: input batch j's network input is allocated (with its
+        RGB channels) when the batch arrives, its parsing channels are filled as the smoother releases its frames, and it is
+        synthesised once all of them are in"""
+        raft_model, window, iters = self.smoothing
+        sm = smooth_parsing.ParsingSmoother(raft_model, window, iters)
+        net = self.parsing_net
+        waiting = collections.deque()       # [x [B, 22, H, W], index of its first frame, frames filled] in clip order
+        n_in = 0
+
+        def fill(r):
+            for item in waiting:
+                k = r.index - item[1]
+                if 0 <= k < item[0].shape[0]:
+                    r.fuse_down(item[0][k, 3:], 1.0 / 16.0)      # style_transfer.py:174's x_p / 16
+                    item[2] += 1
+                    return
+            raise AssertionError(f"smoothed frame {r.index} has no waiting batch")
+
+        for item in self._uploaded(batches):
+            if isinstance(item, (tuple, list)) or item.dtype != torch.uint8 or item.dim() != 4 or item.shape[3] != 3:
+                raise ValueError("FramePipeline: with smoothing, batches must be uint8 [B, H, W, 3] RGB frames")
+            frames = item
+            if self.prefilter is not None:
+                n_blur, size, crop = self.prefilter
+                frames = ops.frame_prefilter_resize(frames, n_blur, size, crop)
+            B, H, W, _ = frames.shape
+            if H % 8 or W % 8 or H < 64 or W < 64:
+                raise ValueError(f"FramePipeline: smoothing needs frames whose H and W are multiples of 8 and at least 64 (RAFT runs "
+                                 f"at 2H x 2W); got {H}x{W}")
+            x = torch.empty((B, 22, H, W), device=self.device, dtype=torch.float32)
+            ops.frames_u8_to_f32(frames, out=x)                        # channels 0..2: ToTensor + Normalize(0.5, 0.5)
+            waiting.append([x, n_in, 0])
+            n_in += B
+            Is, stem = smooth_parsing.frame_prep(frames)
+            fuse, _, _ = net._features(ops.frame_s2d(ops.frames_u8_to_f32(frames), upsample2=True))
+            Ps = ops.logits_readout(net.conv_out.logits_nhwc(fuse), net.n_classes, 2 * H, 2 * W, step=1)   # parsingpredictor(2*Is)[0]
+            for b in range(B):
+                for r in sm.push(Is[b], Ps[b], stem[b:b + 1]):
+                    fill(r)
+            del Is, stem, Ps
+            while waiting and waiting[0][2] == waiting[0][0].shape[0]:
+                yield self.synthesize(waiting.popleft()[0])
+        if n_in == 0:
+            return
+        for r in sm.finish():
+            fill(r)
+        while waiting:
+            x, _, filled = waiting.popleft()
+            assert filled == x.shape[0]
+            yield self.synthesize(x)
 
 
 # ----------------------------------------------------------------------------------------------

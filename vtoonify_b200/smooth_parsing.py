@@ -17,6 +17,11 @@ The loop streams (DESIGN.md section 12):
     ``Downsample([1, 3, 3, 1], 2)`` launch.  The centre pair RAFT(I_i, I_i) of the script is skipped: the script overwrites both of
     its results.
 The RAFT convolutions follow ``set_precision``; the warp and the fusion are fp32 in every mode.
+
+``ParsingSmoother`` is that loop as a stream (``smooth_parsing_maps`` is a loop over its ``push`` and ``finish``): one frame in, the
+outputs that have become computable out, so neither side holds the clip.  ``FramePipeline(smoothing=...)`` runs it between the face
+parsing and the synthesis, with ``frame_prep`` (uint8 frames -> ``Is`` and RAFT's stem input in one launch) and
+``parsing_fuse_down`` (fusion, ``Downsample`` and the ``/ 16`` of style_transfer.py in one launch) (DESIGN.md section 13).
 """
 import torch
 
@@ -87,15 +92,230 @@ def parsing_fuse(imgs, pars, flows, wt, out=None):
     return out
 
 
-def _check_args(Is, Ps, raft_model, window, iters):
+def parsing_fuse_down(centres, wt, out, scale=1.0):
+    """``len(centres)`` centres of the window fusion, each followed by ``Downsample([1, 3, 3, 1], 2)`` and ``* scale``, in one launch
+    that never writes the fused 2x map: ``centres[b] = (imgs, pars, flows)`` as for :func:`parsing_fuse`, host weights wt, and
+    ``out`` [B, C, H/2, W/2] (each sample contiguous, any batch stride: e.g. ``x[:, 3:]`` of VToonify's input).  Bit-identical to
+    :func:`parsing_fuse`, then ``ops.upfirdn2d_planar`` and ``ops.axpby(.., scale)`` (TF32-rounded under ``set_precision('tf32')``
+    like ``axpby``)."""
+    B = len(centres)
+    if B < 1:
+        raise ValueError("parsing_fuse_down: need at least one centre")
+    n = len(centres[0][0])
+    if n % 2 != 1 or n > 2 * MAX_WINDOW + 1 or len(wt) != n:
+        raise ValueError(f"parsing_fuse_down: need 2 * window + 1 <= {2 * MAX_WINDOW + 1} slots and as many weights")
+    C, H, W = centres[0][1][0].shape
+    for imgs, pars, flows in centres:
+        if len(imgs) != n or len(pars) != n or len(flows) != n:
+            raise ValueError("parsing_fuse_down: every centre needs the same number of slots")
+        for k in range(n):
+            ok = tuple(imgs[k].shape) == (3, H, W) and tuple(pars[k].shape) == (C, H, W)
+            ok = ok and (k == n // 2 or tuple(flows[k].shape) == (2, H, W))
+            if not ok:
+                raise ValueError(f"parsing_fuse_down: slot {k} must hold [3, {H}, {W}], [{C}, {H}, {W}] and [2, {H}, {W}] tensors")
+            ops._req_cuda(imgs[k], pars[k], None if k == n // 2 else flows[k])
+            if not (imgs[k].is_contiguous() and pars[k].is_contiguous() and (k == n // 2 or flows[k].is_contiguous())):
+                raise ValueError(f"parsing_fuse_down: slot {k} tensors must be contiguous")
+    Ho, Wo = H // 2, W // 2
+    ops._req_cuda(out)
+    if (out.dim() != 4 or tuple(out.shape) != (B, C, Ho, Wo) or out.stride()[1:] != (Ho * Wo, Wo, 1)
+            or (B > 1 and out.stride(0) < C * Ho * Wo)):
+        raise ValueError(f"parsing_fuse_down: out must be [{B}, {C}, {Ho}, {Wo}] with contiguous samples (got {tuple(out.shape)}, "
+                         f"strides {out.stride()})")
+    ptrs = [(c_void_p * (B * n))(*[None if t is None else t.data_ptr() for c in centres for t in c[j]]) for j in range(3)]
+    w = (c_float * n)(*[float(v) for v in wt])
+    check(load().vt_parsing_fuse_down_f32(ptrs[0], ptrs[1], ptrs[2], w, n, B, out.data_ptr(), out.stride(0), C, H, W, float(scale),
+                                          ops._round_flag(), ops._stream()))
+    return out
+
+
+def frame_prep(frames: torch.Tensor, cpad: int = 32):
+    """uint8 RGB frames [B, H, W, 3] on the device -> (Is [B, 3, 2H, 2W], stem [B, H, W, cpad]) in one launch: the script's
+    ``F.interpolate(transform(frame), scale_factor=2, mode='bilinear')`` and RAFT's stem input ``raft._input_s2d((Is + 1) * 255.0 / 2)``
+    with the script's three roundings.  The up-sampling is ``ops.frame_s2d``'s: ``frame_s2d(frames_u8_to_f32(frames), upsample2=True)``
+    equals ``frame_s2d(2 * Is, upsample2=False)`` bit for bit."""
+    if not frames.is_cuda or frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+        raise ValueError("frame_prep: frames must be a CUDA uint8 [B, H, W, 3] tensor")
+    frames = frames.contiguous()
+    B, H, W, _ = frames.shape
+    img = torch.empty((B, 3, 2 * H, 2 * W), device=frames.device, dtype=torch.float32)
+    stem = torch.empty((B, H, W, cpad), device=frames.device, dtype=torch.float32)
+    check(load().vt_smooth_frame_prep_u8(frames.data_ptr(), img.data_ptr(), stem.data_ptr(), B, H, W, cpad, ops._stream()))
+    return img, stem
+
+
+def _check_model_window(name, raft_model, window, iters):
     if not isinstance(raft_model, RAFT):
-        raise NotImplementedError("smooth_parsing_maps: raft_model must be a vtoonify_b200.raft.RAFT")
+        raise NotImplementedError(f"{name}: raft_model must be a vtoonify_b200.raft.RAFT")
     raft_model._check_model()
-    _check_no_grad("smooth_parsing_maps", Is, Ps)
     if int(window) != window or window < 0 or window > MAX_WINDOW:
-        raise ValueError(f"smooth_parsing_maps: window must be an integer in 0..{MAX_WINDOW} (got {window})")
+        raise ValueError(f"{name}: window must be an integer in 0..{MAX_WINDOW} (got {window})")
     if int(iters) < 1:
-        raise ValueError("smooth_parsing_maps: iters must be at least 1")
+        raise ValueError(f"{name}: iters must be at least 1")
+
+
+def release_schedule(N: int, window: int):
+    """which outputs :class:`ParsingSmoother` hands back: ``(per_push, at_finish)`` with ``per_push[f]`` the output indices the push of
+    frame f returns (output i once frame i + window is in) and ``at_finish`` the last ``window`` (their tail slots repeat
+    ``Is[-window:]``, known only at the end).  The whole clip's schedule; a push computes its own entry with
+    :func:`released_by_push`."""
+    per_push = [[f - window] if f >= window else [] for f in range(N)]
+    return per_push, list(range(max(N - window, 0), N)) if window else []
+
+
+def released_by_push(f: int, window: int):
+    """the outputs the push of frame f releases, ``release_schedule(N, window)[0][f]`` for any N > f, in O(1)"""
+    return [f - window] if f >= window else []
+
+
+def output_slots(i: int, window: int, N: int = None):
+    """``slot_frames(N, window)[i]`` in O(window): slot k of output i is frame i + k - window, or frame i + k in the head
+    (i + k < window: ``Is[0:w]``); with N given, the tail (i + k >= window + N: ``Is[-w:]``) is frame i + k - 2 * window.  Without N,
+    i must be released before the end of the clip (i + window < N for the clip's N), where the tail is never reached."""
+    out = []
+    for j in range(i, i + 2 * window + 1):
+        if j < window:
+            out.append(j)
+        elif N is None or j < window + N:
+            out.append(j - window)
+        else:
+            out.append(j - 2 * window)
+    return out
+
+
+class SmoothedFrame:
+    """one output frame of :class:`ParsingSmoother`, computable from the ring: ``down()`` gives its parsing map [C, H/2, W/2]
+    (``parsing_fuse`` then ``Downsample``, the route of ``smooth_parsing_maps``), ``fuse_down(out, scale)`` writes ``scale`` times
+    the same map into ``out`` in one launch.  The RAFT flows of the centre run on the first of them.  A handle returned by ``push``
+    is valid until the next ``push``; those returned by ``finish`` stay valid."""
+
+    def __init__(self, smoother, index, pos):
+        self.index = index
+        self._sm, self._pos, self._flows = smoother, pos, None
+        self._pushed = smoother.n            # the ring holds this handle's frames while no further frame is pushed
+
+    def _slots(self):
+        sm, pos = self._sm, self._pos
+        if sm.n != self._pushed:
+            raise RuntimeError(f"SmoothedFrame {self.index}: read after a later push (frame {sm.n - 1}) has overwritten its window; "
+                               "read each handle before pushing the next frame")
+        if self._flows is None:
+            self._flows = sm._flows(self.index, pos)
+        return [sm._img[p] for p in pos], [sm._par[p] for p in pos], self._flows
+
+    def down(self):
+        imgs, pars, flows = self._slots()
+        sm = self._sm
+        parsing_fuse(imgs, pars, flows, sm.wt, out=sm._fused)
+        return ops.upfirdn2d_planar(sm._fused[None], sm._kernel, (1, 1), (2, 2), (1, 1, 1, 1))[0]
+
+    def fuse_down(self, out, scale=1.0):
+        parsing_fuse_down([self._slots()], self._sm.wt, out[None], scale)
+        return out
+
+
+class ParsingSmoother:
+    """The smoothing loop of smooth_parsing_map.py as a stream: ``push(I, P)`` takes one frame's 2x image ``I`` [3, H, W] in [-1, 1] and
+    parsing logits ``P`` [C, H, W] on the device and returns the :class:`SmoothedFrame` handles that have become computable (output i
+    once frame i + window is in); ``finish()`` returns the last ``window`` outputs, whose tail slots repeat the clip's last frames.
+    Device memory is a ring of the ``2 * window + 1`` frames of the current window and does not grow with the clip (DESIGN.md
+    section 12).  ``push(I, P, stem)`` takes RAFT's stem input of ``(I + 1) * 255.0 / 2`` precomputed ([1, H/2, W/2, 32], e.g.
+    from :func:`frame_prep`) instead of computing it.  Each output's cnet state and flows are computed when its handle is first
+    read, so a consumer reads every handle before pushing the next frame: a handle read after a later push raises
+    ``RuntimeError``, and so does a push after ``finish``.  Host work per frame is O(window), whatever the clip's length."""
+
+    def __init__(self, raft_model: RAFT, window: int = 5, iters: int = 20):
+        _check_model_window("ParsingSmoother", raft_model, window, iters)
+        self.model, self.window, self.iters = raft_model, int(window), int(iters)
+        self.R = 2 * self.window + 1
+        self.wt = temporal_weights(self.window).tolist()
+        self.n = 0                          # frames pushed
+        self.finished = False
+        self.flow_sink = None               # tests: flow_sink(i, up) receives output i's up-sampled flows [2 * window, 2, H, W]
+        self._img = None
+
+    def _alloc(self, I, P):
+        R, dev = self.R, I.device
+        C, H, W = P.shape
+        self.shape = (C, H, W)
+        # the ring: frame f lives at position f % R (the frames one output reads span at most R consecutive indices)
+        self._img = torch.empty((R, 3, H, W), device=dev, dtype=torch.float32)
+        self._par = torch.empty((R, C, H, W), device=dev, dtype=torch.float32)
+        self._fmap = [None] * R
+        self._stem = [None] * R             # pushed stem inputs; frames pushed without one keep (I + 1) * 255 / 2 in _rin
+        self._rin = None
+        self._fused = torch.empty((C, H, W), device=dev, dtype=torch.float32)
+        self._kernel = make_kernel([1, 3, 3, 1]).to(dev)
+
+    def push(self, I: torch.Tensor, P: torch.Tensor, stem: torch.Tensor = None):
+        # every argument is checked before any state changes
+        if self.finished:
+            raise RuntimeError("ParsingSmoother.push: the clip has ended (finish() was called)")
+        if I.dim() != 3 or I.shape[0] != 3 or P.dim() != 3 or P.shape[1:] != I.shape[1:]:
+            raise ValueError(f"ParsingSmoother.push: I {tuple(I.shape)} must be [3, H, W] and P {tuple(P.shape)} [C, H, W]")
+        ops._req_cuda(I, P, stem)
+        H, W = I.shape[1:]
+        if H % 8 or W % 8 or H < MIN_SIZE or W < MIN_SIZE:
+            raise ValueError(f"ParsingSmoother.push: H and W must be multiples of 8 and at least {MIN_SIZE} (got {H}x{W})")
+        if self._img is not None and tuple(P.shape) != self.shape:
+            raise ValueError(f"ParsingSmoother.push: P {tuple(P.shape)} differs from the clip's {self.shape}")
+        if stem is not None and (tuple(stem.shape) != (1, H // 2, W // 2, 32) or not stem.is_contiguous()):
+            raise ValueError(f"ParsingSmoother.push: stem must be contiguous [1, {H // 2}, {W // 2}, 32]")
+        if self._img is None:
+            self._alloc(I, P)
+        f, m = self.n, self.model
+        r = f % self.R
+        with torch.no_grad():
+            self._img[r].copy_(I)
+            self._par[r].copy_(P)
+            if self.window:
+                if stem is None:
+                    if self._rin is None:
+                        self._rin = torch.empty_like(self._img)
+                    torch.add(self._img[r], 1, out=self._rin[r]).mul_(255.0).div_(2)    # the script's (I + 1) * 255.0 / 2
+                    self._stem[r] = None
+                    self._fmap[r] = m._features(m._input_s2d(self._rin[r:r + 1]))
+                else:
+                    self._stem[r] = stem
+                    self._fmap[r] = m._features(stem)
+        self.n += 1
+        return [self._ready(i) for i in released_by_push(f, self.window)]
+
+    def finish(self):
+        N = self.n
+        if N < max(self.window, 1):
+            raise ValueError(f"ParsingSmoother: {N} frames are fewer than the window {self.window} (the script's RAFT batches would "
+                             "not match)")
+        self.finished = True
+        return [self._ready(i, N) for i in range(N - self.window, N)]
+
+    def _ready(self, i, N=None):
+        # before the end, output i's slots never reach the tail, so they do not depend on the clip's length
+        return SmoothedFrame(self, i, [f % self.R for f in output_slots(i, self.window, N)])
+
+    def _flows(self, i, pos):
+        """cnet once on the centre, the RAFT iterations on the 2 * window non-centre pairs as one batch (the script's centre pair is
+        skipped: the script overwrites both of its results)"""
+        w, R, m = self.window, self.R, self.model
+        if not w:
+            return [None]
+        c = pos[w]
+        nb = [pos[k] for k in range(R) if k != w]
+        B = len(nb)
+        with torch.no_grad():
+            f1 = self._fmap[c].expand(B, -1, -1, -1).contiguous()
+            f2 = torch.cat([self._fmap[p] for p in nb], 0)
+            stem = self._stem[c] if self._stem[c] is not None else m._input_s2d(self._rin[c:c + 1])
+            net, x = m._context(stem)
+            _, up = m._iterate(f1, f2, net.expand(B, -1, -1, -1).contiguous(), x.expand(B, -1, -1, -1).contiguous(), self.iters)
+        if self.flow_sink is not None:
+            self.flow_sink(i, up)
+        return [up[k if k < w else k - 1] if k != w else None for k in range(R)]
+
+
+def _check_args(Is, Ps, raft_model, window, iters):
+    _check_model_window("smooth_parsing_maps", raft_model, window, iters)
+    _check_no_grad("smooth_parsing_maps", Is, Ps)
     if Is.dim() != 4 or Is.shape[1] != 3 or Ps.dim() != 4 or Ps.shape[0] != Is.shape[0] or Ps.shape[2:] != Is.shape[2:]:
         raise ValueError(f"smooth_parsing_maps: Is {tuple(Is.shape)} must be [N, 3, H, W] and Ps {tuple(Ps.shape)} [N, C, H, W]")
     if Is.dtype != torch.float32 or Ps.dtype != torch.float32:
@@ -113,49 +333,20 @@ def smooth_parsing_maps(Is: torch.Tensor, Ps: torch.Tensor, raft_model: RAFT, wi
 
 
 def _smooth(Is, Ps, raft_model, window, iters, flow_sink=None):
-    """smooth_parsing_maps; ``flow_sink(i, up)`` (tests) receives output frame i's up-sampled flows [2 * window, 2, H, W]"""
+    """smooth_parsing_maps as a loop over ParsingSmoother.push and finish; ``flow_sink(i, up)`` (tests) receives output frame i's
+    up-sampled flows [2 * window, 2, H, W]"""
     _check_args(Is, Ps, raft_model, window, iters)
-    window, iters = int(window), int(iters)
     N, C, H, W = Ps.shape
     dev = Is.device if Is.is_cuda else (Ps.device if Ps.is_cuda else next(raft_model.parameters()).device)
     if dev.type != "cuda":
         raise ValueError("smooth_parsing_maps: the RAFT model (or Is / Ps) must be on a CUDA device")
-    R = 2 * window + 1
-    wt = temporal_weights(window).tolist()
-    slots = slot_frames(N, window)
-    kernel = make_kernel([1, 3, 3, 1]).to(dev)
     parse = torch.empty((N, C, H // 2, W // 2), device=Ps.device, dtype=torch.float32)
+    sm = ParsingSmoother(raft_model, window, iters)
+    sm.flow_sink = flow_sink
     with torch.no_grad():
-        # the ring: frame f lives at position f % R (the frames one output reads span at most R consecutive indices)
-        img = torch.empty((R, 3, H, W), device=dev, dtype=torch.float32)
-        rin = torch.empty((R, 3, H, W), device=dev, dtype=torch.float32)
-        par = torch.empty((R, C, H, W), device=dev, dtype=torch.float32)
-        fmap = [None] * R
-        loaded = -1                       # frames 0..loaded have been uploaded and encoded
-        fused = torch.empty((C, H, W), device=dev, dtype=torch.float32)
-        for i in range(N):
-            fr = slots[i]
-            for f in range(loaded + 1, max(fr) + 1):
-                r = f % R
-                img[r].copy_(Is[f])
-                par[r].copy_(Ps[f])
-                torch.add(img[r], 1, out=rin[r]).mul_(255.0).div_(2)        # the script's (I + 1) * 255.0 / 2
-                if window:
-                    fmap[r] = raft_model._features(raft_model._input_s2d(rin[r:r + 1]))
-                loaded = f
-            pos = [f % R for f in fr]
-            c = pos[window]
-            flows = [None] * R
-            if window:
-                nb = [pos[k] for k in range(R) if k != window]
-                B = len(nb)
-                f1 = fmap[c].expand(B, -1, -1, -1).contiguous()
-                f2 = torch.cat([fmap[p] for p in nb], 0)
-                net, x = raft_model._context(raft_model._input_s2d(rin[c:c + 1]))
-                _, up = raft_model._iterate(f1, f2, net.expand(B, -1, -1, -1).contiguous(), x.expand(B, -1, -1, -1).contiguous(), iters)
-                flows = [up[k if k < window else k - 1] if k != window else None for k in range(R)]
-                if flow_sink is not None:
-                    flow_sink(i, up)
-            parsing_fuse([img[p] for p in pos], [par[p] for p in pos], flows, wt, out=fused)
-            parse[i].copy_(ops.upfirdn2d_planar(fused[None], kernel, (1, 1), (2, 2), (1, 1, 1, 1))[0])
+        for f in range(N):
+            for r in sm.push(Is[f].to(dev), Ps[f].to(dev)):
+                parse[r.index].copy_(r.down())
+        for r in sm.finish():
+            parse[r.index].copy_(r.down())
     return parse

@@ -15,6 +15,8 @@ collective inside the forward.  :class:`ShardedFrameLoop` implements the referen
 the clip, every round it scatters one input batch per rank and gathers the uint8 frames back, over ``torch.distributed``
 (NCCL on NVLink for CUDA tensors, gloo in the CPU tests), overlapped with the synthesis of the neighbouring rounds.
 :func:`scatter_batches` / :func:`gather_frames` are the same collectives in their simple blocking form.
+:class:`ShardedSmoothedVideo` runs smoothed video the same way, one segment of output frames with its halo of neighbouring
+frames per rank (DESIGN.md §14).
 """
 import collections
 import contextlib
@@ -236,17 +238,39 @@ class FramePipeline:
         for x in self._uploaded(batches):
             yield self.process(x)
 
+    def _smoothing_frames(self, item):
+        """a device item of a smoothed run -> its uint8 frames after ``prefilter``, with the checks of the smoothed route"""
+        if isinstance(item, (tuple, list)) or item.dtype != torch.uint8 or item.dim() != 4 or item.shape[3] != 3:
+            raise ValueError("FramePipeline: with smoothing, batches must be uint8 [B, H, W, 3] RGB frames")
+        frames = item
+        if self.prefilter is not None:
+            n_blur, size, crop = self.prefilter
+            frames = ops.frame_prefilter_resize(frames, n_blur, size, crop)
+        _, H, W, _ = frames.shape
+        if H % 8 or W % 8 or H < 64 or W < 64:
+            raise ValueError(f"FramePipeline: smoothing needs frames whose H and W are multiples of 8 and at least 64 (RAFT runs "
+                             f"at 2H x 2W); got {H}x{W}")
+        return frames
+
     def _compute_smoothed(self, batches: Iterable):
-        """one device result per input batch through the streaming smoother: input batch j's network input is allocated (with its
-        RGB channels) when the batch arrives, its parsing channels are filled as the smoother releases its frames, and it is
-        synthesised once all of them are in"""
+        """one device result per input batch through the streaming smoother"""
+        return self._smoothed((self._smoothing_frames(item) for item in self._uploaded(batches)), 0, None, True)
+
+    def _smoothed(self, batches, first, outputs, finish):
+        """the streaming smoother between the face parsing and the synthesis.  ``batches`` yields uint8 frames after ``prefilter`` in
+        clip order from frame ``first``.  A batch whose first frame is in ``outputs`` (a range; None: every frame) is synthesised: its
+        network input is allocated (with its RGB channels) when it arrives, its parsing channels are filled as the smoother releases
+        its frames, and it is yielded once all of them are in.  The other batches (halo frames) are prepped, parsed and pushed only,
+        and the outputs outside ``outputs`` are not read.  ``finish`` ends the stream with ``finish()``."""
         raft_model, window, iters = self.smoothing
-        sm = smooth_parsing.ParsingSmoother(raft_model, window, iters)
+        sm = smooth_parsing.ParsingSmoother(raft_model, window, iters, first)
         net = self.parsing_net
         waiting = collections.deque()       # [x [B, 22, H, W], index of its first frame, frames filled] in clip order
-        n_in = 0
+        n_in = first
 
         def fill(r):
+            if outputs is not None and r.index not in outputs:
+                return
             for item in waiting:
                 k = r.index - item[1]
                 if 0 <= k < item[0].shape[0]:
@@ -255,20 +279,12 @@ class FramePipeline:
                     return
             raise AssertionError(f"smoothed frame {r.index} has no waiting batch")
 
-        for item in self._uploaded(batches):
-            if isinstance(item, (tuple, list)) or item.dtype != torch.uint8 or item.dim() != 4 or item.shape[3] != 3:
-                raise ValueError("FramePipeline: with smoothing, batches must be uint8 [B, H, W, 3] RGB frames")
-            frames = item
-            if self.prefilter is not None:
-                n_blur, size, crop = self.prefilter
-                frames = ops.frame_prefilter_resize(frames, n_blur, size, crop)
+        for frames in batches:
             B, H, W, _ = frames.shape
-            if H % 8 or W % 8 or H < 64 or W < 64:
-                raise ValueError(f"FramePipeline: smoothing needs frames whose H and W are multiples of 8 and at least 64 (RAFT runs "
-                                 f"at 2H x 2W); got {H}x{W}")
-            x = torch.empty((B, 22, H, W), device=self.device, dtype=torch.float32)
-            ops.frames_u8_to_f32(frames, out=x)                        # channels 0..2: ToTensor + Normalize(0.5, 0.5)
-            waiting.append([x, n_in, 0])
+            if outputs is None or n_in in outputs:
+                x = torch.empty((B, 22, H, W), device=self.device, dtype=torch.float32)
+                ops.frames_u8_to_f32(frames, out=x)                    # channels 0..2: ToTensor + Normalize(0.5, 0.5)
+                waiting.append([x, n_in, 0])
             n_in += B
             Is, stem = smooth_parsing.frame_prep(frames)
             fuse, _, _ = net._features(ops.frame_s2d(ops.frames_u8_to_f32(frames), upsample2=True))
@@ -279,14 +295,44 @@ class FramePipeline:
             del Is, stem, Ps
             while waiting and waiting[0][2] == waiting[0][0].shape[0]:
                 yield self.synthesize(waiting.popleft()[0])
-        if n_in == 0:
+        if n_in == first:
             return
-        for r in sm.finish():
-            fill(r)
+        if finish:
+            for r in sm.finish():
+                fill(r)
         while waiting:
             x, _, filled = waiting.popleft()
             assert filled == x.shape[0]
             yield self.synthesize(x)
+
+    def smooth_segment(self, frames_dev: torch.Tensor, seg, batch: int) -> torch.Tensor:
+        """One segment of a smoothed clip (``seg`` from ``smooth_parsing.segment_plan(N, window, length)``): ``frames_dev`` holds the
+        clip's uint8 RGB frames ``[seg.lo, seg.hi)`` on the device, ``[seg.hi - seg.lo, H, W, 3]`` (``prefilter`` applies as in
+        ``run``).  Returns the device uint8 BGR frames of outputs ``[seg.a, seg.b)``, ``[seg.b - seg.a, 4H, 4W, 3]``: the same bytes
+        as those frames of ``run`` over the whole clip in batches of ``batch``, so ``seg.a`` must be a multiple of ``batch`` (a
+        ``length`` that is).  The halo frames are prepped, parsed and pushed, not synthesised (DESIGN.md section 14)."""
+        if self.smoothing is None:
+            raise ValueError("FramePipeline.smooth_segment: the pipeline has no smoothing")
+        window = self.smoothing[1]
+        if not isinstance(seg, smooth_parsing.Segment):
+            raise ValueError("FramePipeline.smooth_segment: seg must be a smooth_parsing.Segment (from segment_plan)")
+        a, b, lo, hi, finish = seg
+        # the plan's halos: window frames before a (fewer at the clip's head), window after b or, with finish, up to the clip's end
+        if not (0 <= lo == max(0, a - window) and a < b and (b <= hi < b + window if finish else hi == b + window)):
+            raise ValueError(f"FramePipeline.smooth_segment: {seg} is not a segment of a plan with window {window}")
+        if int(batch) != batch or batch < 1 or a % batch:
+            raise ValueError(f"FramePipeline.smooth_segment: batch must be a positive integer that divides the first output {a} "
+                             f"(got {batch})")
+        if (not isinstance(frames_dev, torch.Tensor) or not frames_dev.is_cuda or frames_dev.dtype != torch.uint8
+                or frames_dev.dim() != 4 or frames_dev.shape[0] != hi - lo or frames_dev.shape[3] != 3):
+            raise ValueError(f"FramePipeline.smooth_segment: frames must be a CUDA uint8 [{hi - lo}, H, W, 3] tensor (the segment's "
+                             f"frames {lo}..{hi - 1})")
+        # batches of `batch` frames from a (those of run over the whole clip), the halos cut likewise
+        cuts = sorted({*range(lo, a, int(batch)), *range(a, b, int(batch)), *range(b, hi, int(batch)), hi})
+        batches = (self._smoothing_frames(frames_dev[s - lo:e - lo]) for s, e in zip(cuts[:-1], cuts[1:]))
+        with torch.no_grad():
+            outs = list(self._smoothed(batches, lo, range(a, b), finish))
+        return outs[0] if len(outs) == 1 else torch.cat(outs)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -356,7 +402,8 @@ class ShardedFrameLoop:
     asynchronously and double-buffered: the scatter of round r+1 is in flight while round r is synthesised, the gather of
     round r while round r+1 is; ``fn`` is the only thing on the compute stream.
 
-    ``fn``: device batch -> device result (e.g. ``lambda t: pipe.synthesize(pipe.assemble(t))``).
+    ``fn``: device batch -> device result (e.g. ``lambda t: pipe.synthesize(pipe.assemble(t))``); with ``indexed=True``,
+    ``fn(batch, i)`` also gets the global index ``i`` of the batch.
     ``stage``: rank 0 only, ``stage(i) -> device tensor`` of global batch ``i`` (from host memory: an H2D copy; from device
     memory: a lookup).  ``sink``: rank 0 only, ``sink(i, result_dev, ready)`` — called in order for every global batch once its
     gather has been *issued*; ``ready()`` makes the current stream wait for the data (CUDA) / blocks (CPU).  ``result_dev`` is
@@ -365,8 +412,9 @@ class ShardedFrameLoop:
     Works on CPU tensors with the gloo backend (tests) and on CUDA tensors with NCCL.
     """
 
-    def __init__(self, fn: Callable, in_shape, in_dtype, out_shape, out_dtype, device, group=None, src: int = 0):
-        self.fn, self.group, self.src = fn, group, src
+    def __init__(self, fn: Callable, in_shape, in_dtype, out_shape, out_dtype, device, group=None, src: int = 0,
+                 indexed: bool = False):
+        self.fn, self.group, self.src, self.indexed = fn, group, src, indexed
         self.world, self.rank = dist.get_world_size(group), dist.get_rank(group)
         self.device = torch.device(device)
         self.cuda = self.device.type == "cuda"
@@ -433,7 +481,7 @@ class ShardedFrameLoop:
             if pend_gather[s] is not None:
                 pend_gather[s].wait()                   # the gather of round r-2 has consumed send[s] / filled gath[s]
             if have:
-                out = self.fn(self._recv[s])
+                out = self.fn(self._recv[s], r * self.world + self.rank) if self.indexed else self.fn(self._recv[s])
                 self._send[s].copy_(out)
                 mine += 1
             else:
@@ -461,3 +509,113 @@ class ShardedFrameLoop:
             if w is not None:
                 w.wait()
         return mine
+
+
+class ShardedSmoothedVideo:
+    """Smoothed video over ``world`` GPUs, one process per GPU: the clip's N outputs are cut into segments of ``length`` outputs
+    (``smooth_parsing.segment_plan``), and segment ``r * world + k`` is smoothed and synthesised on rank k by
+    ``pipe.smooth_segment(frames, seg, batch)`` (a ``FramePipeline`` with ``smoothing``), which gives the bytes of the one-GPU
+    ``pipe.run`` over the clip in batches of ``batch``.  Built on :class:`ShardedFrameLoop`: every round, rank 0 scatters one
+    zero-padded ``[length + 2 * window, H, W, 3]`` uint8 segment (its frames with their halos) per rank and gathers the
+    ``[length, 4h, 4w, 3]`` uint8 BGR outputs back (h, w: the frame size after ``prefilter``).
+
+    ``run(frames, sink)`` on rank 0, ``run()`` on the others.  ``frames`` is an iterable of the clip's N uint8 RGB frames, each item
+    one ``[H, W, 3]`` frame or a batch ``[n, H, W, 3]``, read once and in order; rank 0 keeps the 2 * window frames the next
+    segment's halo shares with the last one, so its host and device memory are bounded by ``world``, ``length`` and the frame size,
+    whatever N (DESIGN.md section 14).  ``sink(i, frames, ready)`` is called in clip order, once per segment, with the segment's
+    first output index ``i`` and its device frames ``[b - a, 4h, 4w, 3]``, with the contract of :class:`ShardedFrameLoop`'s sink
+    (``ready()`` before reading; the buffer is reused two rounds later unless the sink returns an event)."""
+
+    def __init__(self, pipe, N: int, length: int, frame_shape, batch: int, device, group=None, src: int = 0):
+        if pipe.smoothing is None:
+            raise ValueError("ShardedSmoothedVideo: the pipeline has no smoothing")
+        window = pipe.smoothing[1]
+        self.plan = smooth_parsing.segment_plan(N, window, length)
+        if int(batch) != batch or batch < 1 or length % batch:
+            raise ValueError(f"ShardedSmoothedVideo: length {length} must be a multiple of the batch size (got {batch}), so that "
+                             "every batch holds the frames it holds in the one-GPU run")
+        if len(frame_shape) != 2 or any(int(s) != s or s < 1 for s in frame_shape):
+            raise ValueError(f"ShardedSmoothedVideo: frame_shape must be (H, W) (got {frame_shape})")
+        self.pipe, self.N, self.length, self.batch = pipe, int(N), int(length), int(batch)
+        self.frame_shape = tuple(int(s) for s in frame_shape)
+        H, W = self.frame_shape
+        if pipe.prefilter is None:
+            h, w = H, W
+        else:
+            _, (dw, dh), crop = pipe.prefilter
+            top, bottom, left, right = (0, dh, 0, dw) if crop is None else crop
+            h, w = bottom - top, right - left
+        self.loop = ShardedFrameLoop(self._segment, (self.length + 2 * window, H, W, 3), torch.uint8, (self.length, 4 * h, 4 * w, 3),
+                                     torch.uint8, device, group=group, src=src, indexed=True)
+
+    def _segment(self, x, i):
+        seg = self.plan[i]
+        out = self.pipe.smooth_segment(x[:seg.hi - seg.lo], seg, self.batch)
+        if out.shape[0] < self.length:                # the clip's last segment
+            out = torch.cat([out, out.new_zeros((self.length - out.shape[0],) + tuple(out.shape[1:]))])
+        return out
+
+    def run(self, frames: Optional[Iterable] = None, sink: Optional[Callable] = None) -> int:
+        """Smooth and synthesise the clip; returns the number of segments this rank computed."""
+        loop = self.loop
+        if loop.rank != loop.src:
+            return loop.run(len(self.plan))
+        if frames is None or sink is None:
+            raise ValueError("ShardedSmoothedVideo.run: rank 0 needs the clip's frames and a sink")
+        reader = _HaloReader(frames, self.N, self.frame_shape)
+        plan, cuda = self.plan, loop.cuda
+
+        def stage(i):
+            seg = plan[i]
+            buf = torch.empty(loop.in_shape, dtype=torch.uint8, pin_memory=cuda)
+            n = seg.hi - seg.lo
+            buf[n:].zero_()
+            for f in range(seg.lo, seg.hi):
+                buf[f - seg.lo].copy_(reader.frame(f))
+            reader.drop_before(plan[i + 1].lo if i + 1 < len(plan) else self.N)
+            return buf.to(loop.device, non_blocking=True)
+
+        def seg_sink(i, buf, ready):
+            a, b = plan[i].a, plan[i].b
+            return sink(a, buf[:b - a], ready)
+
+        return loop.run(len(plan), stage=stage, sink=seg_sink)
+
+
+class _HaloReader:
+    """rank 0's view of the clip for :class:`ShardedSmoothedVideo`: frames read once, in order, from an iterable of ``[H, W, 3]``
+    frames or ``[n, H, W, 3]`` batches; it holds copies of the frames from the oldest one still needed"""
+
+    def __init__(self, frames: Iterable, N: int, frame_shape):
+        self.it, self.N, self.shape = iter(frames), N, tuple(frame_shape) + (3,)
+        self.kept = collections.deque()              # copies of frames base, base + 1, ...
+        self.base = 0
+        self.item, self.off = None, 0
+
+    def _read(self):
+        f = self.base + len(self.kept)
+        while self.item is None or self.off == self.item.shape[0]:
+            item = next(self.it, None)
+            if item is None:
+                raise ValueError(f"ShardedSmoothedVideo: the clip ended after {f} frames; {self.N} were announced")
+            item = torch.as_tensor(item)
+            if item.dim() == 3:
+                item = item[None]
+            if item.dtype != torch.uint8 or item.dim() != 4 or tuple(item.shape[1:]) != self.shape:
+                raise ValueError(f"ShardedSmoothedVideo: frames must be uint8 {list(self.shape)} or batches [n, "
+                                 f"{', '.join(map(str, self.shape))}] (got {item.dtype} {list(item.shape)})")
+            if f + item.shape[0] > self.N:
+                raise ValueError(f"ShardedSmoothedVideo: the clip has more than the {self.N} frames announced")
+            self.item, self.off = item, 0
+        self.kept.append(self.item[self.off].clone())
+        self.off += 1
+
+    def frame(self, f: int) -> torch.Tensor:
+        while self.base + len(self.kept) <= f:
+            self._read()
+        return self.kept[f - self.base]
+
+    def drop_before(self, f: int):
+        while self.kept and self.base < f:
+            self.kept.popleft()
+            self.base += 1

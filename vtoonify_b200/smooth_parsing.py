@@ -22,7 +22,11 @@ The RAFT convolutions follow ``set_precision``; the warp and the fusion are fp32
 outputs that have become computable out, so neither side holds the clip.  ``FramePipeline(smoothing=...)`` runs it between the face
 parsing and the synthesis, with ``frame_prep`` (uint8 frames -> ``Is`` and RAFT's stem input in one launch) and
 ``parsing_fuse_down`` (fusion, ``Downsample`` and the ``/ 16`` of style_transfer.py in one launch) (DESIGN.md section 13).
+``segment_plan`` cuts a clip into segments that smooth independently, each pushing its frames and a halo of ``window`` frames on
+each side into a ``ParsingSmoother(first=...)`` (DESIGN.md section 14).
 """
+import collections
+
 import torch
 
 from . import ops
@@ -163,9 +167,42 @@ def release_schedule(N: int, window: int):
     return per_push, list(range(max(N - window, 0), N)) if window else []
 
 
-def released_by_push(f: int, window: int):
-    """the outputs the push of frame f releases, ``release_schedule(N, window)[0][f]`` for any N > f, in O(1)"""
-    return [f - window] if f >= window else []
+def released_by_push(f: int, window: int, first: int = 0):
+    """the outputs the push of frame f releases, ``release_schedule(N, window)[0][f]`` for any N > f, in O(1).  For a stream whose
+    first frame is ``first``, only the outputs whose slots are all pushed: those with i >= first + window when first > 0."""
+    i = f - window
+    return [i] if i >= 0 and max(0, i - window) >= first else []
+
+
+def released_at_finish(N: int, window: int, first: int = 0):
+    """the outputs ``finish()`` releases for a clip of N frames, ``release_schedule(N, window)[1]``; for a stream whose first frame is
+    ``first``, only those whose slots are all pushed, as for :func:`released_by_push`"""
+    return list(range(max(N - window, first + window if first else 0), N))
+
+
+Segment = collections.namedtuple("Segment", "a b lo hi finish")
+Segment.__doc__ = """one segment of :func:`segment_plan`: outputs ``[a, b)``, frames ``[lo, hi)`` pushed into a
+``ParsingSmoother(first=lo)``, and whether the segment ends with ``finish()`` (then ``hi`` is the clip's N)"""
+
+
+def segment_plan(N: int, window: int, length: int):
+    """Cut the outputs ``0..N-1`` of a clip into consecutive segments of ``length`` outputs (the last may be shorter) that can be
+    smoothed independently: a segment pushes its outputs' frames and up to ``window`` frames on each side (its halo), so every slot of
+    its outputs is pushed.  A segment with a tail output (``i + window >= N``, released only by ``finish()``) pushes to the clip's
+    end and calls ``finish()``.  Returns a list of :class:`Segment` (DESIGN.md section 14)."""
+    if int(N) != N or int(window) != window or window < 0 or window > MAX_WINDOW:
+        raise ValueError(f"segment_plan: N must be an integer and window an integer in 0..{MAX_WINDOW} (got {N}, {window})")
+    if int(length) != length or length < 1:
+        raise ValueError(f"segment_plan: length must be a positive integer (got {length})")
+    N, window, length = int(N), int(window), int(length)
+    if N < max(window, 1):
+        raise ValueError(f"segment_plan: {N} frames are fewer than the window {window} (the script's RAFT batches would not match)")
+    plan = []
+    for a in range(0, N, length):
+        b = min(a + length, N)
+        finish = b - 1 + window >= N
+        plan.append(Segment(a, b, max(0, a - window), N if finish else b + window, finish))
+    return plan
 
 
 def output_slots(i: int, window: int, N: int = None):
@@ -222,11 +259,18 @@ class ParsingSmoother:
     section 12).  ``push(I, P, stem)`` takes RAFT's stem input of ``(I + 1) * 255.0 / 2`` precomputed ([1, H/2, W/2, 32], e.g.
     from :func:`frame_prep`) instead of computing it.  Each output's cnet state and flows are computed when its handle is first
     read, so a consumer reads every handle before pushing the next frame: a handle read after a later push raises
-    ``RuntimeError``, and so does a push after ``finish``.  Host work per frame is O(window), whatever the clip's length."""
+    ``RuntimeError``, and so does a push after ``finish``.  Host work per frame is O(window), whatever the clip's length.
 
-    def __init__(self, raft_model: RAFT, window: int = 5, iters: int = 20):
+    ``first`` numbers the pushed frames from that clip index (a segment of :func:`segment_plan`): output i is released only once every
+    frame of its slots is in, i.e. i >= first + window when first > 0, and ``finish()`` applies the tail rule to the clip's
+    N = first + frames pushed."""
+
+    def __init__(self, raft_model: RAFT, window: int = 5, iters: int = 20, first: int = 0):
         _check_model_window("ParsingSmoother", raft_model, window, iters)
+        if int(first) != first or first < 0:
+            raise ValueError(f"ParsingSmoother: first must be a non-negative integer (got {first})")
         self.model, self.window, self.iters = raft_model, int(window), int(iters)
+        self.first = int(first)
         self.R = 2 * self.window + 1
         self.wt = temporal_weights(self.window).tolist()
         self.n = 0                          # frames pushed
@@ -263,7 +307,7 @@ class ParsingSmoother:
             raise ValueError(f"ParsingSmoother.push: stem must be contiguous [1, {H // 2}, {W // 2}, 32]")
         if self._img is None:
             self._alloc(I, P)
-        f, m = self.n, self.model
+        f, m = self.first + self.n, self.model
         r = f % self.R
         with torch.no_grad():
             self._img[r].copy_(I)
@@ -279,15 +323,15 @@ class ParsingSmoother:
                     self._stem[r] = stem
                     self._fmap[r] = m._features(stem)
         self.n += 1
-        return [self._ready(i) for i in released_by_push(f, self.window)]
+        return [self._ready(i) for i in released_by_push(f, self.window, self.first)]
 
     def finish(self):
-        N = self.n
+        N = self.first + self.n
         if N < max(self.window, 1):
             raise ValueError(f"ParsingSmoother: {N} frames are fewer than the window {self.window} (the script's RAFT batches would "
                              "not match)")
         self.finished = True
-        return [self._ready(i, N) for i in range(N - self.window, N)]
+        return [self._ready(i, N) for i in released_at_finish(N, self.window, self.first)]
 
     def _ready(self, i, N=None):
         # before the end, output i's slots never reach the tail, so they do not depend on the clip's length

@@ -483,6 +483,31 @@ int vt_frame_blur4_u8(const uint8_t* in, uint8_t* out, int B, int H, int W, void
 int vt_frame_resize_crop_u8(const uint8_t* in, uint8_t* out, int B, int Hs, int Ws, int dh, int dw, int top, int left,
                             int Ho, int Wo, const int* xtab, const int* ytab, void* stream);
 
+/* ---- f2: FFHQ face alignment (align_all_parallel.py:108-147; vtoonify_b200.align), byte for byte with Pillow / NumPy / SciPy --- */
+/* Images are uint8 RGB [H, W, 3] with a row pitch in bytes (a crop is a pointer offset); pad = host int[4] (left, top, right, bottom),
+ * each >= 1; the padded image is [H + top + bottom, W + left + right, 3]. */
+#define VT_ALIGN_MAX_RADIUS 127
+/* one axis of Pillow resize(LANCZOS): horizontal -> out [H, out_size, 3], else out [out_size, W, 3] (contiguous).  tab: device int32
+ * [out_size] first tap, [out_size] tap count, [out_size * ksize] 22-bit fixed-point taps (vtoonify_b200.align.lanczos_table) */
+int vt_align_lanczos_u8(const uint8_t* in, int64_t in_pitch, int H, int W, uint8_t* out, int out_size, int horizontal, const int* tab,
+                        int ksize, void* stream);
+/* axis 0 of scipy.ndimage.gaussian_filter ('reflect') over np.pad(float32(in), pad, 'reflect'): out float32 [Hp, Wp, 3];
+ * w: host double [r + 1], the centre tap first */
+int vt_align_blur_rows_f32(const uint8_t* in, int64_t in_pitch, int H, int W, const int* pad, float* out, const double* w, int r,
+                           void* stream);
+/* axis 1 of the same Gaussian: in, out float32 [Hp, Wp, 3]; with img (the image under the pad; else NULL, and H, W, pad unread) out is
+ * the first blend padded + (g - padded) * clip(3 mask + 1, 0, 1) instead of g */
+int vt_align_blur_cols_f32(const float* in, float* out, int Hp, int Wp, const double* w, int r, const uint8_t* img, int64_t img_pitch,
+                           int H, int W, const int* pad, void* stream);
+/* device workspace of vt_align_median_f32 */
+int64_t vt_align_median_ws_bytes(void);
+/* med (device float32 [3]) = np.median(x, axis=0) of x [n, 3] float32 */
+int vt_align_median_f32(const float* x, int64_t n, float* med, void* ws, void* stream);
+/* out uint8 [Hp, Wp, 3] = clip(rint(x + (med - x) * clip(mask, 0, 1)), 0, 255); x float32 [Hp, Wp, 3], med device float32 [3] */
+int vt_align_finish_u8(const float* x, const float* med, uint8_t* out, int Hp, int Wp, const int* pad, void* stream);
+/* Pillow transform((size, size), QUAD, corners, BILINEAR): out [size, size, 3]; coef: host double[8], the QUAD coefficients */
+int vt_align_warp_u8(const uint8_t* in, int64_t in_pitch, int H, int W, const double* coef, uint8_t* out, int size, void* stream);
+
 /* ---- a11: frame loop transforms ----------------------------------------------------------- */
 /* u8 HWC (RGB or BGR) -> fp32 NCHW in [-1,1]: (v/255 - 0.5)/0.5 ; style_transfer.py:57-60,110,160 */
 int vt_frame_u8_to_f32(const uint8_t* in, float* out, int B, int H, int W, int swap_rb, int64_t out_batch_stride, void* stream);

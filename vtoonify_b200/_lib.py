@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvtoonify_b200.so")
 ABI_VERSION = 7
 VT_MAX_TAPS = 36
+VT_ALIGN_MAX_RADIUS = 127   # include/vtoonify_b200.h: the longest Gaussian half-kernel of the alignment's blur
 ACT_NONE, ACT_LRELU, ACT_RELU_TANH = 0, 1, 2
 
 
@@ -150,6 +151,13 @@ SYMBOLS = {
     "vt_axpby_f32": (c_int, [_P, _P, _P, c_int64, c_float, c_float, c_int, _P]),
     "vt_frame_blur4_u8": (c_int, [_P, _P, c_int, c_int, c_int, _P]),
     "vt_frame_resize_crop_u8": (c_int, [_P, _P] + [c_int] * 9 + [_P, _P, _P]),
+    "vt_align_lanczos_u8": (c_int, [_P, c_int64, c_int, c_int, _P, c_int, c_int, _P, c_int, _P]),
+    "vt_align_blur_rows_f32": (c_int, [_P, c_int64, c_int, c_int, _P, _P, _P, c_int, _P]),
+    "vt_align_blur_cols_f32": (c_int, [_P, _P, c_int, c_int, _P, c_int, _P, c_int64, c_int, c_int, _P, _P]),
+    "vt_align_median_ws_bytes": (c_int64, []),
+    "vt_align_median_f32": (c_int, [_P, c_int64, _P, _P, _P]),
+    "vt_align_finish_u8": (c_int, [_P, _P, _P, c_int, c_int, _P, _P]),
+    "vt_align_warp_u8": (c_int, [_P, c_int64, c_int, c_int, _P, _P, c_int, _P]),
     "vt_frame_u8_to_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int64, _P]),
     "vt_f32_to_frame_u8": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
 }

@@ -434,6 +434,15 @@ int vt_raft_corr_pool_f32(const float* in, float* out, int64_t N, int h, int w, 
  * zeros outside (grid_sample, align_corners=True) */
 int vt_raft_corr_lookup_f32(const float* const* levels, const int64_t* strides, int h2, int w2, const float* coords, float* out,
                             int out_cpitch, int64_t npix, void* stream);
+/* F.avg_pool2d(2, 2) of an NHWC feature map in [B, h, w, C] -> dense out [B, h/2, w/2, C] (floor), torch's summation order;
+ * C % 4 == 0, both 16-byte aligned */
+int vt_raft_fmap_pool_f32(const float* in, float* out, int B, int h, int w, int C, void* stream);
+/* the lookup of vt_raft_corr_lookup_f32 without the correlation volume (AlternateCorrBlock): fmap1 [B, h, w, 256] (batch stride
+ * fmap1_bstride floats, 0 allowed; rows dense), fmap2_levels[l] dense [B, h >> l, w >> l, 256] (fmap2 and its 2x2 mean pools),
+ * coords [B, h, w, 2] (x, y) -> out[p * out_cpitch + l*81 + 9i + j] = the bilinear tap at coords[p] / 2^l + (i - 4, j - 4) of
+ * fmap1[p] . fmap2_l / 16 (zeros outside), channels 324..out_cpitch-1 = 0; fp32 FMA in every precision mode; h, w >= 8 */
+int vt_raft_corr_ondemand_f32(const float* fmap1, int64_t fmap1_bstride, const float* const* fmap2_levels, int B, int h, int w,
+                              const float* coords, float* out, int out_cpitch, void* stream);
 /* out [B, h, w, Cout] = relu(bias + 7x7 convolution (zero padding 3) of the flow coords - grid); w: [7*7][2][Cout] */
 int vt_raft_convf1_f32(const float* coords, const float* w, const float* bias, float* out, int B, int h, int wd, int Cout, void* stream);
 /* coords [B, h, w, 2] (x, y) = (init ? pixel grid : coords) + delta (planar [B, 2, h, w], may be NULL); flow_out (may be NULL) gets

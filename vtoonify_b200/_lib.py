@@ -121,6 +121,8 @@ SYMBOLS = {
     "vt_raft_context_f32": (c_int, [_P, _P, _P, c_int64, c_int, c_int, _P]),
     "vt_raft_corr_pool_f32": (c_int, [_P, _P, c_int64, c_int, c_int, c_int64, _P]),
     "vt_raft_corr_lookup_f32": (c_int, [POINTER(c_void_p), POINTER(c_int64), c_int, c_int, _P, _P, c_int, c_int64, _P]),
+    "vt_raft_fmap_pool_f32": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+    "vt_raft_corr_ondemand_f32": (c_int, [_P, c_int64, POINTER(c_void_p), c_int, c_int, c_int, _P, _P, c_int, _P]),
     "vt_raft_convf1_f32": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     "vt_raft_flow_f32": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P]),
     "vt_raft_gru_reset_f32": (c_int, [_P, _P, _P, c_int64, c_int, _P]),

@@ -5,6 +5,9 @@
 //   raft_context     cnet's split: tanh(net) into the GRU state, relu(inp) into the GRU input buffer
 //   raft_corr_pool   F.avg_pool2d(corr, 2, 2) over the (h2, w2) axes of every correlation row (floor sizes, torch's summation order)
 //   raft_corr_lookup CorrBlock.__call__: 4 levels x 81 bilinear taps (grid_sample, align_corners=True, zeros outside)
+//   raft_fmap_pool   F.avg_pool2d(fmap, 2, 2) of an NHWC feature map (floor sizes, torch's summation order): the on-demand pyramid
+//   raft_corr_ondemand  the same 4 x 81 taps without the all-pairs volume (AlternateCorrBlock): per pixel and level the dot products of
+//                    fmap1 with the pooled fmap2 at the 10 x 10 integer positions around floor(coords / 2^l) - 4, combined bilinearly
 //   raft_convf1      the motion encoder's 7x7 convolution of the 2-channel flow (49 taps: a direct kernel) + bias + ReLU
 //   raft_flow        coords1 (+)= delta, or the flow coords1 - coords0 written into a channel slice of an NHWC buffer
 //   raft_gru_reset / raft_gru_update   sigmoid(r) * h, and h = (1 - sigmoid(z)) h + sigmoid(z) tanh(q)
@@ -139,6 +142,127 @@ raft_corr_lookup_kernel(Pyramid pyr, const float* __restrict__ coords, float* __
   }
 }
 
+// out [B, h/2, w/2, C] = 2x2 means of in [B, h, w, C] (floor sizes, C % 4 == 0); ((a00 + a01) + a10) + a11, then / 4, as ATen
+__global__ void __launch_bounds__(256)
+raft_fmap_pool_kernel(const float4* __restrict__ in, float4* __restrict__ out, int h, int w, int C4, int64_t total) {
+  const int ho = h / 2, wo = w / 2;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C4);
+    int64_t t = i / C4;
+    const int x = (int)(t % wo);
+    t /= wo;
+    const int y = (int)(t % ho);
+    const int64_t b = t / ho;
+    const float4* p = in + ((b * h + 2 * y) * w + 2 * x) * C4 + c;
+    const float4 a = __ldg(p), bb = __ldg(p + C4), cc = __ldg(p + (int64_t)w * C4), d = __ldg(p + (int64_t)w * C4 + C4);
+    float4 s;
+    s.x = 0.f; s.x += a.x; s.x += bb.x; s.x += cc.x; s.x += d.x;
+    s.y = 0.f; s.y += a.y; s.y += bb.y; s.y += cc.y; s.y += d.y;
+    s.z = 0.f; s.z += a.z; s.z += bb.z; s.z += cc.z; s.z += d.z;
+    s.w = 0.f; s.w += a.w; s.w += bb.w; s.w += cc.w; s.w += d.w;
+    out[i] = make_float4(s.x / 4.f, s.y / 4.f, s.z / 4.f, s.w / 4.f);
+  }
+}
+
+constexpr int FEAT_C = 256;                   // fnet's output channels
+constexpr int OD_SIDE = WIN + 1;              // 10 integer positions per axis cover the 9 taps and their right / lower neighbours
+constexpr int OD_POS = OD_SIDE * OD_SIDE;     // 100
+constexpr int OD_WARPS = 8;
+
+struct FeatPyramid {
+  const float* lvl[LEVELS];                   // [B, h >> l, w >> l, 256] dense
+  int h[LEVELS], w[LEVELS];
+};
+
+// one step of a reduce-scatter over the warp: lanes that differ in bit OFF exchange halves of v[0, 2 OFF) and keep v[s] = the pair's sum of
+// slot s + (lane & OFF); after the steps 16, 8, 4, 2, 1, lane k holds in v[0] the warp's sum of slot k
+template <int OFF>
+__device__ __forceinline__ void butterfly_step(float (&v)[32], int lane) {
+  const bool up = lane & OFF;
+#pragma unroll
+  for (int s = 0; s < OFF; ++s) {
+    const float send = up ? v[s] : v[s + OFF];
+    const float keep = up ? v[s + OFF] : v[s];
+    v[s] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
+  }
+}
+
+// One warp per pixel p (all four levels); lane k holds channels 4k..4k+3 and 128+4k..128+4k+3 of fmap1[p] in registers.  Per level the
+// 100 dot products fmap1[p] . fmap2_l[by + i, bx + j] ((bx, by) = floor(coords / 2^l) - 4) are taken 32 at a time: each lane sums its
+// 8 channels of every position (fp32 FMA chains), then a butterfly reduce-scatter over the lanes leaves position g*32 + k's sum in lane k
+// (31 shuffles per 32 positions).  Positions outside the map are 0, as grid_sample's zero padding makes them.  The taps then combine
+// four of the warp's dots with the lookup kernel's weights, in its order, and scale by 1/16.  The 8 warps of a CTA take consecutive
+// pixels, so with coherent flows their windows share rows in L1.
+__global__ void __launch_bounds__(OD_WARPS * 32)
+raft_corr_ondemand_kernel(const float* __restrict__ f1, int64_t f1_bstride, FeatPyramid f2, const float* __restrict__ coords,
+                          float* __restrict__ out, int out_cpitch, int64_t hw, int64_t npix) {
+  __shared__ float dots[OD_WARPS][OD_POS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* dw = dots[warp];
+  for (int64_t p = (int64_t)blockIdx.x * OD_WARPS + warp; p < npix; p += (int64_t)gridDim.x * OD_WARPS) {
+    const int64_t b = p / hw;
+    const float* a = f1 + b * f1_bstride + (p - b * hw) * FEAT_C;
+    const float4 a0 = __ldg(reinterpret_cast<const float4*>(a) + lane), a1 = __ldg(reinterpret_cast<const float4*>(a + 128) + lane);
+    const float2 cxy = __ldg(reinterpret_cast<const float2*>(coords) + p);
+    float* o = out + p * out_cpitch;
+    for (int l = 0; l < LEVELS; ++l) {
+      const float inv = 1.f / (float)(1 << l);
+      const float cx = cxy.x * inv, cy = cxy.y * inv;
+      const float bxf = floorf(cx) - (float)RADIUS, byf = floorf(cy) - (float)RADIUS;
+      const int H = f2.h[l], W = f2.w[l];
+      // the window [bx, bx + 9] x [by, by + 9] misses the map (or the coordinate is not finite): every tap is 0
+      if (!(bxf >= -(float)(OD_SIDE - 1) && bxf <= (float)(W - 1) && byf >= -(float)(OD_SIDE - 1) && byf <= (float)(H - 1))) {
+        for (int k = lane; k < WIN * WIN; k += 32) o[l * (WIN * WIN) + k] = 0.f;
+        continue;
+      }
+      const int bx = (int)bxf, by = (int)byf;
+      const float* m = f2.lvl[l] + b * (int64_t)H * W * FEAT_C;
+      for (int g = 0; g * 32 < OD_POS; ++g) {
+        float v[32];
+#pragma unroll
+        for (int s = 0; s < 32; ++s) {
+          const int q = g * 32 + s;
+          const int Y = by + q / OD_SIDE, X = bx + q % OD_SIDE;
+          float d = 0.f;
+          if (q < OD_POS && Y >= 0 && Y < H && X >= 0 && X < W) {           // warp-uniform
+            const float4* r = reinterpret_cast<const float4*>(m + ((int64_t)Y * W + X) * FEAT_C);
+            const float4 b0 = __ldg(r + lane), b1 = __ldg(r + 32 + lane);
+            d = a0.x * b0.x;
+            d = fmaf(a0.y, b0.y, d); d = fmaf(a0.z, b0.z, d); d = fmaf(a0.w, b0.w, d);
+            d = fmaf(a1.x, b1.x, d); d = fmaf(a1.y, b1.y, d); d = fmaf(a1.z, b1.z, d); d = fmaf(a1.w, b1.w, d);
+          }
+          v[s] = d;
+        }
+        butterfly_step<16>(v, lane);
+        butterfly_step<8>(v, lane);
+        butterfly_step<4>(v, lane);
+        butterfly_step<2>(v, lane);
+        butterfly_step<1>(v, lane);
+        if (g * 32 + lane < OD_POS) dw[g * 32 + lane] = v[0];
+      }
+      __syncwarp();
+      for (int k = lane; k < WIN * WIN; k += 32) {
+        const int di = k / WIN - RADIUS, dj = k % WIN - RADIUS;
+        const float ix = cx + (float)di, iy = cy + (float)dj;
+        const float fx = floorf(ix), fy = floorf(iy);
+        const float tx = ix - fx, ty = iy - fy;
+        // floor(ix) is floor(cx) + di, or one more where ix rounded up to an integer: jx in [0, 9], and jx + 1 == 10 only where tx == 0
+        const int jx = (int)fx - bx, jy = (int)fy - by;
+        const bool xr = jx + 1 < OD_SIDE, yr = jy + 1 < OD_SIDE;
+        const float* d = dw + jy * OD_SIDE + jx;
+        float v = 0.f;
+        v += d[0] * ((1.f - tx) * (1.f - ty));
+        if (xr) v += d[1] * (tx * (1.f - ty));
+        if (yr) v += d[OD_SIDE] * ((1.f - tx) * ty);
+        if (xr && yr) v += d[OD_SIDE + 1] * (tx * ty);
+        o[l * (WIN * WIN) + k] = v * (1.f / 16.f);                 // / sqrt(256), exact
+      }
+      __syncwarp();
+    }
+    for (int k = LOOKUP_C + lane; k < out_cpitch; k += 32) o[k] = 0.f;
+  }
+}
+
 // out [B, h, w, Cout] = relu(bias + conv7x7(flow)), flow = coords1 - coords0 (2 channels, zero padding 3); w: [49][2][Cout]
 __global__ void __launch_bounds__(256)
 raft_convf1_kernel(const float* __restrict__ coords, const float* __restrict__ wt, const float* __restrict__ bias,
@@ -258,6 +382,7 @@ raft_upsample_kernel(const float* __restrict__ mask, int mask_cpitch, const floa
 }
 
 bool al8(const void* p) { return ((uintptr_t)p & 7) == 0; }
+bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
 }  // namespace
 
@@ -308,6 +433,33 @@ extern "C" int vt_raft_corr_lookup_f32(const float* const* levels, const int64_t
   }
   const int64_t total = npix * LOOKUP_C;
   raft_corr_lookup_kernel<<<grid1(total, 256), 256, 0, (cudaStream_t)stream>>>(pyr, coords, out, out_cpitch, total);
+  VT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int vt_raft_fmap_pool_f32(const float* in, float* out, int B, int h, int w, int C, void* stream) {
+  VT_CHECK(in && out && B >= 1 && h >= 2 && w >= 2 && C >= 4 && C % 4 == 0 && al16(in) && al16(out),
+           "raft_fmap_pool: bad args (h, w >= 2, C a multiple of 4, 16-byte aligned rows)");
+  const int64_t total = (int64_t)B * (h / 2) * (w / 2) * (C / 4);
+  raft_fmap_pool_kernel<<<grid1(total, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float4*>(in),
+                                                                               reinterpret_cast<float4*>(out), h, w, C / 4, total);
+  VT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int vt_raft_corr_ondemand_f32(const float* fmap1, int64_t fmap1_bstride, const float* const* fmap2_levels, int B, int h,
+                                         int w, const float* coords, float* out, int out_cpitch, void* stream) {
+  VT_CHECK(fmap1 && fmap2_levels && coords && out && B >= 1 && (h >> (LEVELS - 1)) >= 1 && (w >> (LEVELS - 1)) >= 1 &&
+               out_cpitch >= LOOKUP_C && al16(fmap1) && fmap1_bstride >= 0 && fmap1_bstride % 4 == 0 && al8(coords),
+           "raft_corr_ondemand: bad args (h, w >= 8, fmap1 16-byte aligned with a batch stride of 0 or a multiple of 4)");
+  FeatPyramid f2;
+  for (int l = 0; l < LEVELS; ++l) {
+    VT_CHECK(fmap2_levels[l] && al16(fmap2_levels[l]), "raft_corr_ondemand: fmap2 level %d is NULL or not 16-byte aligned", l);
+    f2.lvl[l] = fmap2_levels[l]; f2.h[l] = h >> l; f2.w[l] = w >> l;
+  }
+  const int64_t npix = (int64_t)B * h * w;
+  raft_corr_ondemand_kernel<<<grid1(npix, OD_WARPS), OD_WARPS * 32, 0, (cudaStream_t)stream>>>(fmap1, fmap1_bstride, f2, coords, out,
+                                                                                            out_cpitch, (int64_t)h * w, npix);
   VT_LAUNCH_CHECK();
   return 0;
 }

@@ -51,7 +51,10 @@ _options = {"fold_upconv": 128, "fuse_torgb": True, "fuse_mask_mul": True, "smal
             "rsu_conv": True, "rsu_max_cin": 128,
             # fuse_stats: AdaIN statistics of a conv output come from the producing kernel's epilogue (per-tile partial sums + finalize)
             # instead of a separate pass over the tensor
-            "fuse_stats": True}
+            "fuse_stats": True,
+            # raft_corr: RAFT's correlation lookup from the all-pairs volume ("volume": the pyramid of fmap1 . fmap2, O((h*w)^2) memory)
+            # or computed at each lookup from fmap1 and the pooled fmap2 ("on_demand": AlternateCorrBlock, O(h*w*256) memory)
+            "raft_corr": "volume"}
 if _os.environ.get("VT_FOLD_UPCONV_MAX_CIN"):
     _options["fold_upconv"] = int(_os.environ["VT_FOLD_UPCONV_MAX_CIN"])
 
@@ -70,6 +73,8 @@ def set_option(name: str, value) -> None:
         raise KeyError(name)
     if name == "rs_fmt" and value not in ("bf16", "f16"):
         raise ValueError("split_fmt must be 'bf16' or 'f16'")
+    if name == "raft_corr" and value not in ("volume", "on_demand"):
+        raise ValueError("raft_corr must be 'volume' or 'on_demand'")
     _options[name] = value
 
 

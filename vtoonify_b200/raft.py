@@ -10,8 +10,13 @@ The forward keeps every activation NHWC on the library's kernels (DESIGN.md sect
   * both encoders: the 7x7 / 2 stem as a 4x4 convolution over the space-to-depth tensor of ``2 * (x / 255) - 1`` (normalised before
     the stem's zero padding), ``cnet``'s BatchNorm folded into weights and bias with ReLU and the residual add in the epilogue,
     ``fnet``'s instance norm from the convolution's own statistics, applied with the ReLU (and shortcut) by one elementwise pass;
-  * the all-pairs correlation: a 1x1 convolution of ``fmap1`` with per-sample weights ``fmap2`` (``Cout = h*w`` padded to 32), the
-    1/16 in the epilogue, then three 2x2 mean pools and the 4 x 81-tap bilinear lookup into the 352-channel input of ``convc1``;
+  * the correlation, by ``ops.set_option("raft_corr", ...)`` (DESIGN.md section 16):
+      - ``"volume"`` (the default, CorrBlock): the all-pairs volume as a 1x1 convolution of ``fmap1`` with per-sample weights
+        ``fmap2`` (``Cout = h*w`` padded to 32), the 1/16 in the epilogue, then three 2x2 mean pools of it and per iteration the
+        4 x 81-tap bilinear lookup into the 352-channel input of ``convc1``; (h*w)^2 floats per pair;
+      - ``"on_demand"`` (AlternateCorrBlock, what ``alternate_corr=True`` selects in the reference): three 2x2 mean pools of
+        ``fmap2`` only, and per iteration one kernel that forms the same taps from the dot products of ``fmap1`` with the pooled
+        ``fmap2`` at the 10 x 10 positions around each tap window (fp32 FMA in every precision mode); h*w*256 floats per level;
   * per iteration: the motion encoder writes into channels 128..253 of the GRU input ``x = [inp | motion | flow]``; each GRU half
     is one convolution for z|r (stacked weights), the reset gate, one convolution for q and the state update; the flow head ends in
     a planar 2-channel convolution whose output the coordinate update adds;
@@ -189,7 +194,8 @@ class RAFT(nn.Module):
         if getattr(args, "mixed_precision", False):
             raise NotImplementedError("RAFT: mixed_precision=True is not supported")
         if self.args.alternate_corr:
-            raise NotImplementedError("RAFT: alternate_corr=True (alt_cuda_corr) is not supported")
+            raise NotImplementedError("RAFT: alternate_corr=True (alt_cuda_corr) is not supported; its on-demand correlation is "
+                                      "ops.set_option('raft_corr', 'on_demand')")
         if self.args.dropout:
             raise NotImplementedError("RAFT: dropout > 0 is not supported")
         self.fnet = BasicEncoder(output_dim=256, norm_fn="instance", dropout=args.dropout)
@@ -363,22 +369,33 @@ class RAFT(nn.Module):
 
     def _iterate(self, fmap1, fmap2, net, x, iters, flow_init=None, test_mode=True):
         """the iteration step: correlation pyramid of (fmap1, fmap2) [B, h, w, 256], ``iters`` updates of the GRU state ``net`` and
-        input ``x`` (both updated in place), mask head and convex up-sampling; returns what ``forward`` returns"""
+        input ``x`` (both updated in place), mask head and convex up-sampling; returns what ``forward`` returns.  With
+        ``raft_corr="on_demand"`` fmap1 may have batch stride 0 (one map for every pair, as ``expand`` gives)."""
         lib, st = load(), ops._stream()
         B, h, w, _ = fmap1.shape
         H, W = 8 * h, 8 * w
         dev = fmap1.device
         ub = self.update_block
 
+        on_demand = ops.get_option("raft_corr") == "on_demand"
         with ops.nvtx_range("raft.correlation"):
-            levels = self._pyramid(fmap1, fmap2, B, h, w)
+            if on_demand:
+                if fmap1.stride()[1:] != (w * 256, 256, 1):
+                    fmap1 = fmap1.contiguous()
+                levels = self._fmap_pyramid(fmap2)
+            else:
+                levels = self._pyramid(fmap1, fmap2, B, h, w)
 
         coords = torch.empty((B, h, w, 2), device=dev, dtype=torch.float32)
         fi = None if flow_init is None else flow_init.contiguous()
         check(lib.vt_raft_flow_f32(coords.data_ptr(), ops._ptr(fi), 1, None, 2, B, h, w, st))
-        corr = torch.zeros((B, h, w, CORR_CPAD), device=dev, dtype=torch.float32)
-        lv_ptr = (c_void_p * 4)(*[t.data_ptr() for t, _, _, _ in levels])
-        lv_stride = (c_int64 * 4)(*[s for _, s, _, _ in levels])
+        if on_demand:
+            corr = torch.empty((B, h, w, CORR_CPAD), device=dev, dtype=torch.float32)        # the kernel writes the pad channels
+            lv_ptr = (c_void_p * 4)(*[t.data_ptr() for t in levels])
+        else:
+            corr = torch.zeros((B, h, w, CORR_CPAD), device=dev, dtype=torch.float32)
+            lv_ptr = (c_void_p * 4)(*[t.data_ptr() for t, _, _, _ in levels])
+            lv_stride = (c_int64 * 4)(*[s for _, s, _, _ in levels])
         npix = B * h * w
         x_motion = (128, h * w * 256, w * 256, 256)
         t15, t51, t3, t1 = rect_taps(1, 5), rect_taps(5, 1), ops.conv_taps(3, 1), ops.conv_taps(1, 0)
@@ -404,7 +421,12 @@ class RAFT(nn.Module):
         low = None
         with ops.nvtx_range("raft.iterations"):
             for itr in range(iters):
-                check(lib.vt_raft_corr_lookup_f32(lv_ptr, lv_stride, h, w, coords.data_ptr(), corr.data_ptr(), CORR_CPAD, npix, st))
+                if on_demand:
+                    check(lib.vt_raft_corr_ondemand_f32(fmap1.data_ptr(), fmap1.stride(0), lv_ptr, B, h, w, coords.data_ptr(),
+                                                        corr.data_ptr(), CORR_CPAD, st))
+                else:
+                    check(lib.vt_raft_corr_lookup_f32(lv_ptr, lv_stride, h, w, coords.data_ptr(), corr.data_ptr(), CORR_CPAD, npix,
+                                                      st))
                 c = _conv([corr], w_c1, t1, **_relu_epi())
                 c = _conv([c], w_c2, t3, **_relu_epi())
                 f = torch.empty((B, h, w, 128), device=dev, dtype=torch.float32)
@@ -449,4 +471,16 @@ class RAFT(nn.Module):
             out = torch.empty((N, (hl // 2) * (wl // 2)), device=fmap1.device, dtype=torch.float32)
             check(lib.vt_raft_corr_pool_f32(src.data_ptr(), out.data_ptr(), N, hl, wl, stride, st))
             levels.append((out, (hl // 2) * (wl // 2), hl // 2, wl // 2))
+        return levels
+
+    def _fmap_pyramid(self, fmap2):
+        """the on-demand pyramid: fmap2 [B, h, w, 256] and its three 2x2 mean pools (floor sizes), each dense NHWC"""
+        lib, st = load(), ops._stream()
+        levels = [fmap2.contiguous()]
+        for _ in range(3):
+            src = levels[-1]
+            B, hl, wl, C = src.shape
+            out = torch.empty((B, hl // 2, wl // 2, C), device=src.device, dtype=torch.float32)
+            check(lib.vt_raft_fmap_pool_f32(src.data_ptr(), out.data_ptr(), B, hl, wl, C, st))
+            levels.append(out)
         return levels

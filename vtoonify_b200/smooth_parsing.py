@@ -347,7 +347,9 @@ class ParsingSmoother:
         nb = [pos[k] for k in range(R) if k != w]
         B = len(nb)
         with torch.no_grad():
-            f1 = self._fmap[c].expand(B, -1, -1, -1).contiguous()
+            f1 = self._fmap[c].expand(B, -1, -1, -1)
+            if ops.get_option("raft_corr") != "on_demand":      # the on-demand lookup reads one map at batch stride 0
+                f1 = f1.contiguous()
             f2 = torch.cat([self._fmap[p] for p in nb], 0)
             stem = self._stem[c] if self._stem[c] is not None else m._input_s2d(self._rin[c:c + 1])
             net, x = m._context(stem)
